@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Benchmark of the DDPO hot path on B200 (contract: see the task brief / DESIGN.md §Measurement).
+"""Benchmark of the DDPO hot path on H100 (see DESIGN.md §Measurement).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--phase sample|ppo]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--phase sample|ppo] [--dump-outputs DIR]
 
 Workload = BASELINE.json configs[1]: DDPO, SD2-base 512 px (64x64x4 latents, 77x1024 context), 50-step
 DDIM, CFG 5.0, eta 1.0, per-GPU sample batch 8 (global batch 64 on 8 GPUs), synthetic latents/prompt
@@ -9,17 +9,21 @@ embeddings, random-init U-Net weights.  One bench "step" is one pass of the hot 
   phase=sample : one denoising step of the 8-sample batch (U-Net on the 2x8 CFG batch + fused
                  CFG/DDIM/log-prob/noise kernel)                          -> denoising steps/s
   phase=ppo    : one PPO train pass: 10 timesteps of the train batch of 2 (reference micro-batch, train_cfg) stacked
-                 into one U-Net fwd+bwd of batch 40, log-prob, PPO loss (per-micro-batch means), gradient accumulate;
+                 into one U-Net fwd+bwd of batch 40 (the driver's default train_macro; it fits the 80 GB of an H100), log-prob, PPO loss (per-micro-batch means), gradient accumulate;
                  plus the optimizer update (all-reduce + clip + AdamW) timed separately  -> PPO samples/s
 The headline `value` is PPO samples/s when the training path is available (a PPO sample = 50 sampling
 steps + 50 train steps of one trajectory), else denoising steps/s.
 One process per GPU (torchrun for N>1), max-over-ranks CUDA-event timing.
+--dump-outputs DIR writes, after the timed steps, what the last timed sampling step and the last timed train pass
+computed (latents, log-probs, PPO info, a fixed seeded sample of the accumulated gradient) as DIR/<name>.npy; all inputs
+are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -31,7 +35,7 @@ sys.path.insert(0, ROOT)
 T_STEPS = 50
 SAMPLE_BATCH = 8
 TRAIN_BATCH = 2
-TRAIN_MACRO = int(os.environ.get("DDPO_BENCH_MACRO", "25"))  # timesteps of the same train batch evaluated in one U-Net pass (same parameters, see train_step doc)
+TRAIN_MACRO = int(os.environ.get("DDPO_BENCH_MACRO", "10"))  # timesteps of the same train batch evaluated in one U-Net pass (same parameters, see train_step doc)
 GUIDANCE, ETA, CLIP = 5.0, 1.0, 1e-4
 UNET_GFLOP = 804.3  # algorithmic GFLOP of one SD2-base U-Net application (SURVEY.md §8d / BASELINE.md §2)
 WORKLOAD = "DDPO SD2-base 512px, 50-step DDIM, CFG 5.0, eta 1.0, sample batch 8/GPU (BASELINE configs[1])"
@@ -42,8 +46,8 @@ def _peaks():
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return d.get("bf16_tflops_sustained", 1387.8), d.get("bf16_tflops", 1645.5), d.get("hbm_gbs", 6576.4), "measured"
-    return 1400.0, 1590.0, 6650.0, "fallback"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("bf16_tflops", 989.0), d.get("hbm_gbs", 3350.0), "measured"
+    return 989.0, 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3), not reached"
 
 
 class ClockSampler(threading.Thread):
@@ -182,18 +186,6 @@ def cpu_vae_decode_seconds():
     return time.perf_counter() - t0
 
 
-def _ncu_traffic():
-    """Average DRAM bytes (read + write) per igemm launch of one denoising step, from the committed ncu capture of
-    `bench.py --ncu sample` (profiles/r1_traffic.json, written by profiles/make_launch_summary.py); None if absent."""
-    for name in ("r2_launches_summary.json",):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                return json.load(f)["sample"]["igemm"]["dram_bytes_per_launch"]
-        except Exception:
-            continue
-    return None
-
-
 def _dump_shapes(prof, tags, path):
     """Per-(kernel, shape) table of the eager CUDA-event profile: which GEMM shapes the time goes to."""
     agg = {}
@@ -257,7 +249,7 @@ def cpu_ppo_samples_per_sec(n_denoise):
 def run_reference(args):
     """Reference arm: the reference's own path cannot be installed here (jax / flax / diffusers are absent and there
     is no network, DESIGN.md section 1), so this times the oracle port of it on the host cores -- same metric, unit and
-    workload as the B200 arm.  A timed "step" is ONE U-Net application of one sample (what `ms_per_step` and `steps`
+    workload as the GPU arm.  A timed "step" is ONE U-Net application of one sample (what `ms_per_step` and `steps`
     describe, so steps x ms_per_step is time really spent in this run); one VAE decode and one PPO train step (forward +
     autograd backward through both CFG branches) are timed once each; `value` extrapolates those pieces to a PPO sample
     (`extrapolated: true`): 100 applications + decode + 50 train steps."""
@@ -300,8 +292,10 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--ncu", default="", choices=["", "sample", "train"],
                     help="run under `ncu --profile-from-start off`: bracket ONE eager denoising step / train pass with "
-                         "cudaProfilerStart/Stop, print nothing, exit (profiles/README.md has the command lines)")
+                         "cudaProfilerStart/Stop, print nothing, exit")
     ap.add_argument("--shapes", action="store_true", help="also write per-shape kernel tables to gpurun_out/shapes_*.txt")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write what the last timed sampling step and train pass computed as DIR/<name>.npy")
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"],
                     help="weak: 8 samples per GPU per epoch (default); strong: 64 samples per epoch for the whole job "
                          "(SURVEY 8d: sample batch 8 x 8/N batches per GPU), visible in the epoch-driver e2e number")
@@ -386,6 +380,9 @@ def main():
         dist.barrier()
     ms = e0.elapsed_time(e1)
     sampler.stop_flag = True
+    outputs = {}
+    if args.dump_outputs and rank == 0:
+        outputs = {"sample_latents": S["x_next"].view(B, 4, 64, 64).clone(), "sample_log_probs": S["logp"].clone()}
     tms = torch.tensor([ms], device=dev)
     if world > 1:
         dist.all_reduce(tms, op=dist.ReduceOp.MAX)
@@ -546,9 +543,16 @@ def main():
         t0e, t1e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         t0e.record()
         for i in range(args.steps):
-            pg.train_step(tstate, batches[i % len(batches)], st, sched, True, GUIDANCE, ETA, CLIP, False, micro_batch_size=Bt, pmean_info=False)
+            _, info = pg.train_step(tstate, batches[i % len(batches)], st, sched, True, GUIDANCE, ETA, CLIP, False, micro_batch_size=Bt,
+                                    pmean_info=False)
         t1e.record()
         torch.cuda.synchronize()
+        if args.dump_outputs and rank == 0:
+            for k in ("loss", "approx_kl", "clipfrac"):
+                outputs[f"train_{k}"] = info[k].detach().float().reshape(-1).clone()
+            # the accumulated gradient is ~3.5 GB: 2^20 entries at fixed, seeded positions stand for it
+            gidx = torch.randint(tstate.grad_acc.numel(), (1 << 20,), generator=torch.Generator().manual_seed(0)).to(dev)
+            outputs["train_grad_acc_sample"] = tstate.grad_acc.view(-1)[gidx].clone()
         if world > 1:
             dist.barrier()
         tt = torch.tensor([t0e.elapsed_time(t1e)], device=dev)
@@ -648,9 +652,16 @@ def main():
             argv = ["--dataset", "compressed_animals", "--sample_batch_size", str(B), "--num_sample_batches_per_epoch", str(nsb),
                     "--train_batch_size", str(TRAIN_BATCH), "--train_macro", str(TRAIN_MACRO), "--num_train_epochs", "3",
                     "--save_freq", "1000000", "--savepath", f"bench_driver_{rank}", "--seed", "0"]
-            with contextlib.redirect_stdout(sys.stderr):
-                out = PG.main(argv, models=(pipe, {"unet": net.params, "scheduler": state, "text_encoder": {}}),
-                              max_epochs=3, save_last=False)
+            # the driver writes its logs under the working directory: run it in a temporary one, the tree may be read-only
+            cwd = os.getcwd()
+            with tempfile.TemporaryDirectory(prefix="ddpo_bench_") as tmp:
+                try:
+                    os.chdir(tmp)
+                    with contextlib.redirect_stdout(sys.stderr):
+                        out = PG.main(argv, models=(pipe, {"unet": net.params, "scheduler": state, "text_encoder": {}}),
+                                      max_epochs=3, save_last=False)
+                finally:
+                    os.chdir(cwd)
             # epoch 0 warms up (graph capture, arena growth); of the two steady-state epochs the faster one is reported
             # (the host side -- JPEG threads, Python -- jitters by a few per cent between epochs)
             h = min(out["history"][1:], key=lambda e: e["sample_seconds"] + e["train_seconds"])
@@ -710,7 +721,7 @@ def main():
                        "per_step": "one denoising step of the 8-sample batch (U-Net batch 16)",
                        "samples_per_epoch": "8 per GPU (weak scaling; BASELINE's batch 64 = 8 GPUs x 8; per-sample work is identical)"
                                             if args.scaling == "weak" else "64 over the whole job (strong scaling)",
-                       "l2": "per-step working set (1.7 GB bf16 weights + activations) exceeds the 126 MB L2; no explicit flush",
+                       "l2": "per-step working set (1.7 GB bf16 weights + activations) exceeds the 50 MB L2; no explicit flush",
                        "cuda_graph": True, "per_gpu_steps_per_s": steps_per_s / world,
                        "unet_tflops_per_gpu": step_flops / (ms_per_step * 1e-3) / 1e12},
             "clocks": sampler.summary(),
@@ -731,13 +742,12 @@ def main():
             "ppo": ppo,
             "vae_decode": vae_info,
             "roofline": {"bound": "tensor", "achieved": igemm_tflops, "peak": sus_tf, "unit": "TFLOP/s",
-                         "frac": igemm_tflops / sus_tf, "traffic": _ncu_traffic(), "kernel": "igemm2_kernel (CTA-pair implicit GEMM; igemm_kernel below 1024 rows)",
+                         "frac": igemm_tflops / sus_tf, "kernel": "igemm_kernel (wgmma implicit GEMM)",
                          "peak_source": f"{peak_src} bf16_tflops_sustained",
                          "how": "sum of algorithmic 2MNK over the igemm launches of one step / sum of their CUDA-event durations"},
             "kernels": breakdown,
             "kernels_note": "per-kernel CUDA-event times of ONE EAGER step: every launch carries a few microseconds of event / launch "
-                            "overhead (407 launches per denoising step), so their sum exceeds the graph-replayed ms_per_step; shares "
-                            "are what to compare with the ncu launch lists in profiles/",
+                            "overhead, so their sum exceeds the graph-replayed ms_per_step",
             "cpu_baseline": cpu,
         }
         if ppo is not None and driver is not None and "error" not in driver:
@@ -755,6 +765,12 @@ def main():
                                    "+ 1 optimizer update per 2 samples; a step = one denoising step or one train pass",
                            "samples_per_epoch_per_gpu": nb_}
         line["gpu_mem_peak_gb"] = round(torch.cuda.max_memory_allocated() / 2 ** 30, 2)
+        line["gpu"] = torch.cuda.get_device_name(dev)
+        if args.dump_outputs:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for k, v in outputs.items():
+                np.save(os.path.join(args.dump_outputs, f"{k}.npy"), v.float().cpu().numpy())
+            line["dumped_outputs"] = sorted(outputs)
         print(json.dumps(line))
     # orderly teardown: drop captured graphs and cached buffers before the process exits
     torch.cuda.synchronize()

@@ -1,7 +1,7 @@
-"""Builds ``libddpo_b200.so`` (all CUDA kernels + the C ABI) in-tree with nvcc for sm_100a.
+"""Builds ``libddpo_b200.so`` (all CUDA kernels + the C ABI) in-tree with nvcc for sm_90a (H100).
 
 ``python -m ddpo_b200.build`` or ``__graft_entry__.build()``.  nvcc cross-compiles without
-a GPU; the resulting .so travels with the repo snapshot to the B200 box.
+a GPU; the resulting .so is loaded from the tree.
 """
 import os
 import subprocess
@@ -11,9 +11,9 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libddpo_b200.so")
-SOURCES = ["abi.cu", "igemm.cu", "igemm2.cu", "wgrad.cu", "wgrad2.cu", "attention.cu", "attention_bwd.cu", "norm.cu", "elementwise.cu",
+SOURCES = ["abi.cu", "igemm.cu", "wgrad.cu", "attention.cu", "attention_bwd.cu", "norm.cu", "elementwise.cu",
            "backward_ew.cu", "ddim.cu", "rwr.cu", "vae.cu", "text.cu", "vision.cu", "optim.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -52,7 +52,7 @@ def build(force=False, verbose=False):
 
     with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(compile_one, srcs))
-    cmd = [nvcc, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -5,7 +5,7 @@ post-LayerNorm of the CLS token, visual projection 1024 -> 768), L2 normalisatio
 (``ddpo/models/laion.py:7-18``: five Dense layers 768-1024-128-64-16-1 without activations; dropout is deterministic).
 
 The oracle (``oracle/clip_vision.py``) is pinned against the installed ``transformers`` ``CLIPVisionModelWithProjection``;
-the CUDA path (``csrc/vision.cu`` + the text tower's building blocks) agrees with it within 2e-2 relative on the B200
+the CUDA path (``csrc/vision.cu`` + the text tower's building blocks) agrees with it within 2e-2 relative on the GPU
 (``tests/test_gpu_zz_grouped_temb_aesthetic.py``; full-size ViT-L/14 run included).  Weights are random-init (no checkpoints offline); the
 LAION head loads ``sac+logos+ava1-l14-linearMSE.pth`` from ``cache/`` when the file exists, as the reference does.
 """

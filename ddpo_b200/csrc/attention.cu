@@ -1,31 +1,29 @@
-// Fused softmax attention (forward) on tcgen05, head dim 64 -- self- and cross-attention of the
+// Fused softmax attention (forward) on wgmma (sm_90a), head dim 64 -- self- and cross-attention of the
 // Flax U-Net's BasicTransformerBlock (3P diffusers==0.12.1 attention_flax.py FlaxAttention:
 // S = (Q K^T) * d^-0.5, P = softmax(S), O = P V; reached from the reference at
 // pipeline_flax_stable_diffusion.py:219-224 / training/policy_gradient.py:87-102).
 //
 // The [B*h, N, N] score tensor XLA materialises never exists here.  One CTA owns a 128-query
-// tile of one (sample, head); K/V stream through a 2-stage TMA ring in 128-key blocks:
-//   S_j   = Q K_j^T          tcgen05.mma (SS, both K-major)        -> TMEM  X[j&1] (128 cols fp32)
-//   P_j   = exp2((S_j - m) c)   softmax warps (1 thread = 1 query row, tcgen05.ld), bf16 -> smem
-//   O_j   = P_j V_j          tcgen05.mma (A = P K-major, B = V MN-major) -> TMEM X[j&1][0:64]
-//   O_acc = O_acc * alpha + O_j    in registers (fp32), normalised by the row sum at the end.
-// S_{j+1} is issued before P_j is ready, so QK^T overlaps the softmax; two CTAs are resident
-// per SM (256 TMEM columns, 113 KB shared each) so one CTA's softmax hides the other's MMAs.
+// tile of one (sample, head), two consumer warpgroups of 64 query rows each; K/V stream through a
+// 2-stage TMA ring in 128-key blocks (warp 8 is the producer):
+//   S_j   = Q K_j^T          wgmma m64n128k16 (both operands K-major in shared memory) -> registers
+//   P_j   = exp2((S_j - m) c)   in registers (a quad of threads holds a query row), bf16
+//   O     = O * alpha + P_j V_j   wgmma m64n64k16 with A = P from registers, B = V MN-major
+// normalised by the row sum at the end.  Keys past nk (TMA zero fill) and, with causal masking, keys
+// after the query are masked; key blocks entirely after a causal tile are skipped.
 // Fixed reduction order; no atomics.
 #include "common.cuh"
-#include <stdlib.h>
+#include "wgmma.cuh"
 
 namespace ddpo {
 
-constexpr int AT_THREADS = 192;  // warp0: TMA + TMEM alloc, warp1: MMA, warps 2..5: softmax
+constexpr int AT_THREADS = 288;  // warps 0-7: two consumer warpgroups, warp 8: TMA producer
 constexpr int AT_BQ = 128, AT_BKV = 128, AT_D = 64;
 constexpr int AT_TILE = AT_BQ * AT_D * 2;  // 16 KB: a [128 x 64] bf16 SW128 tile
-constexpr int AT_KV_STAGES = 2;
 constexpr int AT_SMEM_Q = 0;
-constexpr int AT_SMEM_KV = AT_TILE;                                   // stages x (K | V)
-constexpr int AT_SMEM_P = AT_SMEM_KV + AT_KV_STAGES * 2 * AT_TILE;     // 2 tiles (keys 0-63 | 64-127)
-constexpr int AT_SMEM_BAR = AT_SMEM_P + 2 * AT_TILE;
-constexpr int AT_SMEM_TOTAL = AT_SMEM_BAR + 256;
+constexpr int AT_SMEM_KV = AT_TILE;                        // 2 stages x (K | V)
+constexpr int AT_SMEM_BAR = AT_SMEM_KV + 2 * 2 * AT_TILE;
+constexpr int AT_SMEM_TOTAL = AT_SMEM_BAR + 256 + 1024;    // + alignment slack
 
 struct AttnArgs {
   CUtensorMap tmQ, tmK, tmV;
@@ -37,467 +35,138 @@ struct AttnArgs {
   float scale;
 };
 
-__global__ void __launch_bounds__(AT_THREADS, 2) attention_fwd_kernel(const __grid_constant__ AttnArgs p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
+__global__ void __launch_bounds__(AT_THREADS, 1) attention_fwd_kernel(const __grid_constant__ AttnArgs p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + AT_SMEM_BAR);
-  uint64_t* q_full = bars;               // 1
-  uint64_t* kv_full = bars + 1;          // [2]
-  uint64_t* kv_empty = bars + 3;         // [2]
-  uint64_t* s_full = bars + 5;           // [2]
-  uint64_t* o_full = bars + 7;           // [2]
-  uint64_t* x_free = bars + 9;           // [2]
-  uint64_t* p_full = bars + 11;          // 1
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 12);
+  uint64_t* q_full = bars;        // 1
+  uint64_t* kv_full = bars + 1;   // [2]
+  uint64_t* kv_empty = bars + 3;  // [2] (one arrive per consumer warp)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * AT_BQ, head = blockIdx.y, b = blockIdx.z;
-  const int nkb = (p.nk + AT_BKV - 1) / AT_BKV;
+  const int k_end = p.causal ? min(p.nk, q0 + AT_BQ) : p.nk;
+  const int nkb = (k_end + AT_BKV - 1) / AT_BKV;
 
   if (threadIdx.x == 0) {
-    if ((smem_u32(smem) & 1023u) != 0) __trap();  // SW128 tiles need 1024-byte alignment
-    prefetch_tmap(&p.tmQ);
-    prefetch_tmap(&p.tmK);
-    prefetch_tmap(&p.tmV);
     mbar_init(q_full, 1);
     for (int i = 0; i < 2; ++i) {
       mbar_init(&kv_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
-      mbar_init(&s_full[i], 1);
-      mbar_init(&o_full[i], 1);
-      mbar_init(&x_free[i], 4);
+      mbar_init(&kv_empty[i], 8);
     }
-    mbar_init(p_full, 4);
     fence_barrier_init();
   }
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, 256);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // warps 0 / 1 run their loops converged and elect one lane for the TMA / MMA issue only: addresses and descriptors stay
-  // in uniform registers (inside an `if (lane == 0)` region every UTMALDG / UTCHMMA is wrapped in an R2UR + ELECT loop)
-  if (warp == 0) {
-    if (elect_one()) {
+  if (warp == 8) {
+    if (lane == 0) {
+      prefetch_tmap(&p.tmQ);
+      prefetch_tmap(&p.tmK);
+      prefetch_tmap(&p.tmV);
       mbar_expect_tx(q_full, AT_TILE);
       tma_load_4d(smem + AT_SMEM_Q, &p.tmQ, q_full, 0, head, q0, b);
-    }
-    __syncwarp();
-    for (int j = 0; j < nkb; ++j) {
-      const int st = j & 1;
-      mbar_wait(&kv_empty[st], ((j >> 1) & 1) ^ 1);
-      uint8_t* sK = smem + AT_SMEM_KV + st * 2 * AT_TILE;
-      if (elect_one()) {
+      for (int j = 0; j < nkb; ++j) {
+        const int st = j & 1;
+        mbar_wait(&kv_empty[st], ((j >> 1) & 1) ^ 1);
+        uint8_t* sK = smem + AT_SMEM_KV + st * 2 * AT_TILE;
         mbar_expect_tx(&kv_full[st], 2 * AT_TILE);
         tma_load_4d(sK, &p.tmK, &kv_full[st], 0, head, j * AT_BKV, b);
         tma_load_4d(sK + AT_TILE, &p.tmV, &kv_full[st], 0, head, j * AT_BKV, b);
       }
-      __syncwarp();
     }
-  } else if (warp == 1) {
-    {
-      const uint32_t idesc_s = umma_idesc_bf16(AT_BQ, AT_BKV, 0, 0);  // S = Q K^T: N = 128 keys
-      const uint32_t idesc_o = umma_idesc_bf16(AT_BQ, AT_D, 0, 1);    // O = P V : N = 64, B (V) MN-major
-      const uint32_t q_addr = smem_u32(smem + AT_SMEM_Q);
-      const uint32_t p_addr = smem_u32(smem + AT_SMEM_P);
-      auto issue_s = [&](int j) {
-        const int st = j & 1, xb = j & 1;
-        mbar_wait(&x_free[xb], ((j >> 1) & 1) ^ 1);
-        mbar_wait(&kv_full[st], (j >> 1) & 1);
-        tc_fence_after();
-        const uint32_t k_addr = smem_u32(smem + AT_SMEM_KV + st * 2 * AT_TILE);
-        if (elect_one()) {
+    return;
+  }
+
+  // ------------------------------------------------------------ consumer warpgroups
+  // accumulator fragments: thread holds query rows rq[0] = .. + lane / 4 and rq[1] = rq[0] + 8, columns 8 j + 2 (lane & 3) + {0, 1}
+  const int wg = warp >> 2;
+  const int t4 = lane & 3;
+  int rq[2];
+  rq[0] = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  rq[1] = rq[0] + 8;
+  int k_lim[2];  // keys [0, k_lim) are visible to the row (causal: j <= i; key 0 is always visible)
 #pragma unroll
-          for (int k = 0; k < AT_D / 16; ++k)
-            umma_bf16(tmem_base + xb * 128, umma_desc(q_addr + k * 32, 16, 1024), umma_desc(k_addr + k * 32, 16, 1024),
-                      idesc_s, k != 0);
-          umma_commit(&s_full[xb]);
-        }
-        __syncwarp();
-      };
-      mbar_wait(q_full, 0);
-      issue_s(0);
-      for (int j = 0; j < nkb; ++j) {
-        if (j + 1 < nkb) issue_s(j + 1);
-        const int st = j & 1, xb = j & 1;
-        mbar_wait(p_full, j & 1);
-        tc_fence_after();
-        const uint32_t v_addr = smem_u32(smem + AT_SMEM_KV + st * 2 * AT_TILE + AT_TILE);
-        if (elect_one()) {
+  for (int h = 0; h < 2; ++h) k_lim[h] = p.causal ? min(p.nk, rq[h] + 1) : p.nk;
+  const float c = p.scale_log2e;
+  float o[AT_D / 2];
 #pragma unroll
-          for (int k = 0; k < AT_BKV / 16; ++k) {
-            // A = P: K-major, 64-key sub-tiles; B = V: MN-major, 16 keys = 16 rows of 128 B
-            const uint32_t a = p_addr + (k >> 2) * AT_TILE + (k & 3) * 32;
-            const uint32_t bb = v_addr + k * 16 * 128;
-            umma_bf16(tmem_base + xb * 128, umma_desc(a, 16, 1024), umma_desc(bb, 8192, 1024), idesc_o, k != 0);
-          }
-          umma_commit(&o_full[xb]);
-          umma_commit(&kv_empty[st]);
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    // ------------------------------------------------------------ softmax warps
-    const int q = warp & 3;
-    const int r = q * 32 + lane;  // query row within the tile == TMEM lane
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    float o_acc[AT_D];
+  for (int i = 0; i < AT_D / 2; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  const uint32_t q_addr = smem_u32(smem + AT_SMEM_Q) + wg * (64 * 128);
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < nkb; ++j) {
+    const int st = j & 1;
+    mbar_wait(&kv_full[st], (j >> 1) & 1);
+    const uint32_t k_addr = smem_u32(smem + AT_SMEM_KV + st * 2 * AT_TILE), v_addr = k_addr + AT_TILE;
+    float s[AT_BKV / 2];
+    wgmma_fence();
 #pragma unroll
-    for (int i = 0; i < AT_D; ++i) o_acc[i] = 0.f;
-    float m_run = -INFINITY, l_run = 0.f;
-    const float c = p.scale_log2e;
-    uint8_t* sP = smem + AT_SMEM_P;
-    // keys [0, k_lim) are visible to this thread's query row (causal: j <= i; key 0 is always visible)
-    const int k_lim = p.causal ? min(p.nk, q0 + r + 1) : p.nk;
-    // pass 1 of a block: row max over the 128 scores in X[j & 1] (full blocks take the predicate-free path: the
-    // softmax warps are instruction bound)
-    auto row_max = [&](int j) {
-      const int xb = j & 1;
-      mbar_wait(&s_full[xb], (j >> 1) & 1);
-      tc_fence_after();
-      const int valid = min(AT_BKV, k_lim - j * AT_BKV);
-      const bool full = valid == AT_BKV;
-      float m_blk = -INFINITY;
-#pragma unroll 1
-      for (int c0 = 0; c0 < AT_BKV; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(t_lane + xb * 128 + c0, v);
-        tmem_ld_wait();
-        if (full) {
+    for (int k = 0; k < AT_D / 16; ++k)
+      Wgmma<AT_BKV>::ss<0, 0>(s, gmma_desc(q_addr + k * 32, 16, 1024), gmma_desc(k_addr + k * 32, 16, 1024), k != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    const int kbase = j * AT_BKV;
+    uint32_t pa[AT_BKV / 16][4];
 #pragma unroll
-          for (int i = 0; i < 32; ++i) m_blk = fmaxf(m_blk, __uint_as_float(v[i]));
-        } else {
+    for (int h = 0; h < 2; ++h) {
+      const int valid = k_lim[h] - kbase;
+      float mx = -INFINITY;
 #pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (c0 + i < valid) m_blk = fmaxf(m_blk, __uint_as_float(v[i]));
-        }
-      }
-      return m_blk;
-    };
-    // The row max of block j+1 is taken while the tensor core computes P_j V_j, so the wait for O_j is hidden
-    // (it was 14 % of the stall samples when O_j was awaited right after P_j was published).
-    float m_next = row_max(0);
-    for (int j = 0; j < nkb; ++j) {
-      const int xb = j & 1;
-      const int kbase = j * AT_BKV;
-      const int valid = min(AT_BKV, k_lim - kbase);
-      const bool full = valid == AT_BKV;
-      const float m_blk = m_next;
-      const float m_new = fmaxf(m_run, m_blk);
-      const float alpha = ex2_mufu((m_run - m_new) * c);
+      for (int jj = 0; jj < AT_BKV / 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (8 * jj + 2 * t4 + e < valid) mx = fmaxf(mx, s[4 * jj + 2 * h + e]);
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[h], mx);
+      const float alpha = ex2_mufu((m_run[h] - m_new) * c);
       const float mc = m_new * c;
       float l_blk = 0.f;
-      // pass 2: P = exp2(S*c - m*c) -> bf16 -> swizzled smem (K-major SW128, 2 sub-tiles of 64 keys)
-#pragma unroll 1
-      for (int c0 = 0; c0 < AT_BKV; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(t_lane + xb * 128 + c0, v);
-        tmem_ld_wait();
-        float pr[32];
-        if (full) {
 #pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float xe = __uint_as_float(v[i]) * c - mc;
-            pr[i] = ex2_sel<DDPO_EXP_POLY_FWD>(i, xe);
-            l_blk += pr[i];
-          }
-        } else {
+      for (int jj = 0; jj < AT_BKV / 8; ++jj)
 #pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float xe = __uint_as_float(v[i]) * c - mc;
-            const float e = ex2_sel<DDPO_EXP_POLY_FWD>(i, xe);
-            pr[i] = (c0 + i < valid) ? e : 0.f;
-            l_blk += pr[i];
-          }
+        for (int e = 0; e < 2; ++e) {
+          const int col = 8 * jj + 2 * t4 + e;
+          const float pr = col < valid ? ex2_sel<DDPO_EXP_POLY_FWD>(col, s[4 * jj + 2 * h + e] * c - mc) : 0.f;
+          s[4 * jj + 2 * h + e] = pr;
+          l_blk += pr;
         }
-        uint8_t* tile = sP + (c0 >> 6) * AT_TILE + r * 128;
+      l_run[h] = l_run[h] * alpha + l_blk;  // this thread's partial row sum (the quad is summed at the end)
+      m_run[h] = m_new;
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const int chunk = ((c0 & 63) >> 3) + g;  // 16-byte chunk index within the 128-byte row
-          uint4 u;
-          u.x = pack_bf16(pr[g * 8 + 0], pr[g * 8 + 1]);
-          u.y = pack_bf16(pr[g * 8 + 2], pr[g * 8 + 3]);
-          u.z = pack_bf16(pr[g * 8 + 4], pr[g * 8 + 5]);
-          u.w = pack_bf16(pr[g * 8 + 6], pr[g * 8 + 7]);
-          *reinterpret_cast<uint4*>(tile + ((chunk ^ (r & 7)) << 4)) = u;
-        }
-      }
-      l_run = l_run * alpha + l_blk;
-      m_run = m_new;
-      // S consumed + P visible to the tensor core (generic -> async proxy)
-      tc_fence_before();
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-      if (j + 1 < nkb) m_next = row_max(j + 1);
-      // O_j
-      mbar_wait(&o_full[xb], (j >> 1) & 1);
-      tc_fence_after();
+      for (int jj = 0; jj < AT_D / 8; ++jj) o[4 * jj + 2 * h] *= alpha, o[4 * jj + 2 * h + 1] *= alpha;
+    }
 #pragma unroll
-      for (int c0 = 0; c0 < AT_D; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(t_lane + xb * 128 + c0, v);
-        tmem_ld_wait();
+    for (int kk = 0; kk < AT_BKV / 16; ++kk) {
+      pa[kk][0] = pack_bf16(s[8 * kk + 0], s[8 * kk + 1]);
+      pa[kk][1] = pack_bf16(s[8 * kk + 2], s[8 * kk + 3]);
+      pa[kk][2] = pack_bf16(s[8 * kk + 4], s[8 * kk + 5]);
+      pa[kk][3] = pack_bf16(s[8 * kk + 6], s[8 * kk + 7]);
+    }
+    wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < 32; ++i) o_acc[c0 + i] = o_acc[c0 + i] * alpha + __uint_as_float(v[i]);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&x_free[xb]);
-    }
-    const int row = q0 + r;
-    if (row < p.nq) {
-      const float inv = 1.0f / l_run;
-      __nv_bfloat16* o = p.out + (static_cast<size_t>(b) * p.nq + row) * p.ldo + head * AT_D;
-#pragma unroll
-      for (int i = 0; i < AT_D; i += 8) {
-        uint4 u;
-        u.x = pack_bf16(o_acc[i] * inv, o_acc[i + 1] * inv);
-        u.y = pack_bf16(o_acc[i + 2] * inv, o_acc[i + 3] * inv);
-        u.z = pack_bf16(o_acc[i + 4] * inv, o_acc[i + 5] * inv);
-        u.w = pack_bf16(o_acc[i + 6] * inv, o_acc[i + 7] * inv);
-        *reinterpret_cast<uint4*>(o + i) = u;
-      }
-      if (p.lse != nullptr)
-        p.lse[(static_cast<size_t>(b) * p.heads + head) * p.nq + row] = m_run * p.scale + logf(l_run);
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// Cross-attention forward (Nk <= 128 keys: the 77 text tokens).  One 128-query tile is a single key block, so the general
-// kernel above spends its time on per-CTA fixed costs (TMEM allocation, barrier set-up, K/V fetch, pipeline fill and
-// drain for ONE block: 59 us for 84 MB of Q + O traffic at batch 16, 1.4 TB/s).  Here a CTA keeps K and V of its
-// (sample, head) resident and STREAMS query tiles through a 2-stage TMA ring; S_{i+1} = Q_{i+1} K^T is issued while the
-// softmax warps work on tile i, and only the columns that can hold keys are touched: S is a 128 x KB UMMA (KB = keys
-// rounded up to 16), the softmax walks ceil(KB / 32) chunks, P V runs KB / 16 k-steps.  No running max / rescale: one
-// block is the whole row.  Arithmetic per element and summation order are those of the general kernel (the dropped
-// columns / k-steps only ever contributed exact zeros) -> bit-identical outputs, same LSE.
-// The kernel is bound by HBM (77 FLOP per byte of Q + O: at most 0.31 of the bf16 tensor peak at the 6.58 TB/s copy rate).
-constexpr int AX_SMEM_K = 0, AX_SMEM_V = AT_TILE, AX_SMEM_Q = 2 * AT_TILE, AX_SMEM_P = 4 * AT_TILE, AX_SMEM_BAR = 6 * AT_TILE,
-              AX_SMEM_TOTAL = AX_SMEM_BAR + 256;
-
-__global__ void __launch_bounds__(AT_THREADS, 2) attention_cross_fwd_kernel(const __grid_constant__ AttnArgs p, int tiles_per_cta) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + AX_SMEM_BAR);
-  uint64_t* kv_full = bars;              // 1
-  uint64_t* q_full = bars + 1;           // [2]
-  uint64_t* q_empty = bars + 3;          // [2]
-  uint64_t* s_full = bars + 5;           // [2]
-  uint64_t* o_full = bars + 7;           // [2]
-  uint64_t* x_free = bars + 9;           // [2]
-  uint64_t* p_full = bars + 11;          // 1
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 12);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int head = blockIdx.y, b = blockIdx.z;
-  const int n_qtiles = (p.nq + AT_BQ - 1) / AT_BQ;
-  const int t0 = blockIdx.x * tiles_per_cta;
-  const int nt = min(tiles_per_cta, n_qtiles - t0);   // >= 1 by construction of the grid
-  const int KB = (p.nk + 15) & ~15;                   // key columns the tensor core sees (multiple of 16, <= 128)
-  const int nchunk = (KB + 31) >> 5;                  // 32-column softmax chunks that can hold a key
-
-  if (threadIdx.x == 0) {
-    if ((smem_u32(smem) & 1023u) != 0) __trap();
-    prefetch_tmap(&p.tmQ);
-    prefetch_tmap(&p.tmK);
-    prefetch_tmap(&p.tmV);
-    mbar_init(kv_full, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&q_full[i], 1);
-      mbar_init(&q_empty[i], 1);
-      mbar_init(&s_full[i], 1);
-      mbar_init(&o_full[i], 1);
-      mbar_init(&x_free[i], 4);
-    }
-    mbar_init(p_full, 4);
-    fence_barrier_init();
-  }
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, 256);
-    tmem_relinquish();
-  }
-  // P columns >= 32 * nchunk are never written by the softmax warps but are read by no k-step either (k-steps cover KB
-  // <= 32 * nchunk columns); columns in [nk, 32 * nchunk) are written as zeros every tile.
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp == 0) {   // converged loops, elected issue (see attention_fwd_kernel)
-    if (elect_one()) {
-      mbar_expect_tx(kv_full, 2 * AT_TILE);
-      tma_load_4d(smem + AX_SMEM_K, &p.tmK, kv_full, 0, head, 0, b);   // rows >= nk are zero-filled by TMA
-      tma_load_4d(smem + AX_SMEM_V, &p.tmV, kv_full, 0, head, 0, b);
-    }
+    for (int kk = 0; kk < AT_BKV / 16; ++kk)  // B = V: MN-major, 16 keys = 16 rows of 128 B
+      Wgmma<AT_D>::rs<1>(o, pa[kk], gmma_desc(v_addr + kk * 16 * 128, 8192, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
     __syncwarp();
-    for (int i = 0; i < nt; ++i) {
-      const int st = i & 1;
-      mbar_wait(&q_empty[st], ((i >> 1) & 1) ^ 1);
-      if (elect_one()) {
-        mbar_expect_tx(&q_full[st], AT_TILE);
-        tma_load_4d(smem + AX_SMEM_Q + st * AT_TILE, &p.tmQ, &q_full[st], 0, head, (t0 + i) * AT_BQ, b);
-      }
-      __syncwarp();
-    }
-  } else if (warp == 1) {
-    {
-      const uint32_t idesc_s = umma_idesc_bf16(AT_BQ, KB, 0, 0);     // S = Q K^T, N = KB key columns
-      const uint32_t idesc_o = umma_idesc_bf16(AT_BQ, AT_D, 0, 1);   // O = P V, B (V) MN-major
-      const uint32_t k_addr = smem_u32(smem + AX_SMEM_K), v_addr = smem_u32(smem + AX_SMEM_V);
-      const uint32_t p_addr = smem_u32(smem + AX_SMEM_P);
-      auto issue_s = [&](int i) {
-        const int st = i & 1, xb = i & 1;
-        mbar_wait(&x_free[xb], ((i >> 1) & 1) ^ 1);
-        mbar_wait(&q_full[st], (i >> 1) & 1);
-        tc_fence_after();
-        const uint32_t q_addr = smem_u32(smem + AX_SMEM_Q + st * AT_TILE);
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < AT_D / 16; ++k)
-            umma_bf16(tmem_base + xb * 128, umma_desc(q_addr + k * 32, 16, 1024), umma_desc(k_addr + k * 32, 16, 1024),
-                      idesc_s, k != 0);
-          umma_commit(&s_full[xb]);
-          umma_commit(&q_empty[st]);   // the Q tile is free once these MMAs have read it
-        }
-        __syncwarp();
-      };
-      mbar_wait(kv_full, 0);
-      issue_s(0);
-      for (int i = 0; i < nt; ++i) {
-        if (i + 1 < nt) issue_s(i + 1);
-        const int xb = i & 1;
-        mbar_wait(p_full, i & 1);
-        tc_fence_after();
-        if (elect_one()) {
-          for (int k = 0; k < KB / 16; ++k) {
-            const uint32_t a = p_addr + (k >> 2) * AT_TILE + (k & 3) * 32;
-            const uint32_t bb = v_addr + k * 16 * 128;
-            umma_bf16(tmem_base + xb * 128, umma_desc(a, 16, 1024), umma_desc(bb, 8192, 1024), idesc_o, k != 0);
-          }
-          umma_commit(&o_full[xb]);
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    const int r = q * 32 + lane;
-    const uint32_t t_lane = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    const float c = p.scale_log2e;
-    uint8_t* sP = smem + AX_SMEM_P;
-    const int nk = p.nk;
-    auto row_max = [&](int i) {
-      const int xb = i & 1;
-      mbar_wait(&s_full[xb], (i >> 1) & 1);
-      tc_fence_after();
-      float m_blk = -INFINITY;
-#pragma unroll 1
-      for (int c0 = 0; c0 < nchunk * 32; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(t_lane + xb * 128 + c0, v);
-        tmem_ld_wait();
-        if (c0 + 32 <= nk) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) m_blk = fmaxf(m_blk, __uint_as_float(v[j]));
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (c0 + j < nk) m_blk = fmaxf(m_blk, __uint_as_float(v[j]));
-        }
-      }
-      return m_blk;
-    };
-    float m_next = row_max(0);
-    for (int i = 0; i < nt; ++i) {
-      const int xb = i & 1;
-      const float m_row = m_next;
-      const float mc = m_row * c;
-      float l_row = 0.f;
-#pragma unroll 1
-      for (int c0 = 0; c0 < nchunk * 32; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(t_lane + xb * 128 + c0, v);
-        tmem_ld_wait();
-        float pr[32];
-        if (c0 + 32 <= nk) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            pr[j] = ex2_sel<DDPO_EXP_POLY_FWD>(j, __uint_as_float(v[j]) * c - mc);
-            l_row += pr[j];
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const float e = ex2_sel<DDPO_EXP_POLY_FWD>(j, __uint_as_float(v[j]) * c - mc);
-            pr[j] = (c0 + j < nk) ? e : 0.f;
-            l_row += pr[j];
-          }
-        }
-        uint8_t* tile = sP + (c0 >> 6) * AT_TILE + r * 128;
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const int chunk = ((c0 & 63) >> 3) + g;
-          uint4 u;
-          u.x = pack_bf16(pr[g * 8 + 0], pr[g * 8 + 1]);
-          u.y = pack_bf16(pr[g * 8 + 2], pr[g * 8 + 3]);
-          u.z = pack_bf16(pr[g * 8 + 4], pr[g * 8 + 5]);
-          u.w = pack_bf16(pr[g * 8 + 6], pr[g * 8 + 7]);
-          *reinterpret_cast<uint4*>(tile + ((chunk ^ (r & 7)) << 4)) = u;
-        }
-      }
-      tc_fence_before();
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-      if (i + 1 < nt) m_next = row_max(i + 1);
-      mbar_wait(&o_full[xb], (i >> 1) & 1);
-      tc_fence_after();
-      const int row = (t0 + i) * AT_BQ + r;
-      // the general kernel's arithmetic: O_acc = 0 * alpha + O (alpha = exp2(-inf) = 0 on the first block), then * (1 / l)
-      const float inv = 1.0f / l_row;
-      __nv_bfloat16* o = p.out + (static_cast<size_t>(b) * p.nq + row) * p.ldo + head * AT_D;
-#pragma unroll
-      for (int c0 = 0; c0 < AT_D; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(t_lane + xb * 128 + c0, v);
-        tmem_ld_wait();
-        if (row < p.nq) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            uint4 u;
-            u.x = pack_bf16(__uint_as_float(v[j]) * inv, __uint_as_float(v[j + 1]) * inv);
-            u.y = pack_bf16(__uint_as_float(v[j + 2]) * inv, __uint_as_float(v[j + 3]) * inv);
-            u.z = pack_bf16(__uint_as_float(v[j + 4]) * inv, __uint_as_float(v[j + 5]) * inv);
-            u.w = pack_bf16(__uint_as_float(v[j + 6]) * inv, __uint_as_float(v[j + 7]) * inv);
-            *reinterpret_cast<uint4*>(o + c0 + j) = u;
-          }
-        }
-      }
-      if (row < p.nq && p.lse != nullptr)
-        p.lse[(static_cast<size_t>(b) * p.heads + head) * p.nq + row] = m_row * p.scale + logf(l_row);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&x_free[xb]);
-    }
+    if (lane == 0) mbar_arrive(&kv_empty[st]);
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float l = l_run[h];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const int row = rq[h];
+    if (row < p.nq) {
+      const float inv = 1.0f / l;
+      __nv_bfloat16* out = p.out + (static_cast<size_t>(b) * p.nq + row) * p.ldo + head * AT_D + 2 * t4;
+#pragma unroll
+      for (int jj = 0; jj < AT_D / 8; ++jj)
+        *reinterpret_cast<uint32_t*>(out + 8 * jj) = pack_bf16(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
+      if (p.lse != nullptr && t4 == 0)
+        p.lse[(static_cast<size_t>(b) * p.heads + head) * p.nq + row] = m_run[h] * p.scale + logf(l);
+    }
   }
 }
 
@@ -536,31 +205,6 @@ extern "C" int ddpo_attention_fwd(const ddpo_attention_args* a, void* stream) {
     attr = true;
   }
   const int n_qtiles = (a->nq + AT_BQ - 1) / AT_BQ;
-  const char* gen = getenv("DDPO_ATTN_GENERAL");   // developer switch: force the general kernel (bit-identity test, A/B timing)
-  if (a->nk <= AT_BKV && !p.causal && n_qtiles >= 2 && !(gen != nullptr && gen[0] == '1')) {
-    // cross-attention: K/V resident, query tiles streamed.  CTAs per (sample, head) so that the grid is ~2-4 CTAs per SM
-    static bool xattr = false;
-    if (!xattr) {
-      DDPO_CUDA_OK(cudaFuncSetAttribute(attention_cross_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, AX_SMEM_TOTAL));
-      xattr = true;
-    }
-    // CTAs per (sample, head): minimise waves x (tiles per CTA + ~1.5 tiles of fixed cost) with 2 CTAs resident per SM
-    const int pairs = a->heads * a->batch, slots = 2 * num_sms();
-    int split = 1;
-    double best = 1e30;
-    for (int s = 1; s <= n_qtiles; ++s) {
-      const int tpc = (n_qtiles + s - 1) / s;
-      const int ctas = pairs * ((n_qtiles + tpc - 1) / tpc);
-      const double cost = static_cast<double>((ctas + slots - 1) / slots) * (tpc + 1.5);
-      if (cost < best - 1e-9) best = cost, split = s;
-    }
-    const int tiles_per_cta = (n_qtiles + split - 1) / split;
-    split = (n_qtiles + tiles_per_cta - 1) / tiles_per_cta;   // no empty CTAs
-    dim3 xgrid(split, a->heads, a->batch);
-    attention_cross_fwd_kernel<<<xgrid, AT_THREADS, AX_SMEM_TOTAL, static_cast<cudaStream_t>(stream)>>>(p, tiles_per_cta);
-    DDPO_LAUNCH_OK();
-    return DDPO_OK;
-  }
   dim3 grid(n_qtiles, a->heads, a->batch);
   attention_fwd_kernel<<<grid, AT_THREADS, AT_SMEM_TOTAL, static_cast<cudaStream_t>(stream)>>>(p);
   DDPO_LAUNCH_OK();

@@ -1,4 +1,4 @@
-// Attention backward on tcgen05 (head dim 64): the hand-written counterpart of what
+// Attention backward on wgmma (sm_90a, head dim 64): the hand-written counterpart of what
 // `jax.grad(compute_loss)` (reference ddpo/training/policy_gradient.py:138) derives for
 // FlaxAttention (3P diffusers attention_flax.py):  P = softmax(Q K^T / sqrt(d)), O = P V.
 //
@@ -6,20 +6,25 @@
 //   dP = dO V^T ; dS = P * (dP - delta) / sqrt(d)
 //   dV = P^T dO ; dK = dS^T Q ; dQ = dS K
 //
-// Two deterministic kernels (no atomics): `dkdv` owns a 128-key block and streams the query
-// blocks, accumulating dK/dV in TMEM; `dq` owns a 128-query block and streams the key blocks,
-// accumulating dQ in TMEM.  P is recomputed from the saved log-sum-exp (never stored).
-// P / dS tiles are written once to shared memory as [query rows][64 keys] 128-byte swizzled rows and
-// consumed both as a K-major operand (dS K) and as an MN-major operand (P^T dO, dS^T Q).
+// Two deterministic kernels (no atomics): `dkdv` owns a 128-key block and streams 64-query
+// blocks, accumulating dK/dV in registers; `dq` owns a 128-query block and streams 64-key blocks,
+// accumulating dQ in registers.  P is recomputed from the saved log-sum-exp (never stored).
+// Each kernel has two consumer warpgroups (64 rows each) and a TMA producer warp (warp 8).  The
+// score-shaped tiles (S^T / dP^T in dkdv, S / dP in dq) are wgmma accumulators; P and dS go from
+// those registers straight into the A operand of the next wgmma (P^T dO, dS^T Q, dS K), whose B
+// operand is the streamed tile read MN-major.
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace ddpo {
 
-constexpr int AB_THREADS = 320;  // warp0 TMA + TMEM alloc, warp1 MMA, warps 2..9 softmax/epilogue (2 per TMEM lane quarter)
-constexpr int AB_T = 128 * 64 * 2;  // one [128 x 64] bf16 tile
+constexpr int AB_THREADS = 288;      // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int AB_T = 128 * 64 * 2;   // one [128 x 64] bf16 tile
+constexpr int AB_H = 64 * 64 * 2;    // one [64 x 64] bf16 tile
 
 struct AttnBwdArgs {
-  CUtensorMap tmQ, tmK, tmV, tmDO, tmK64, tmV64;  // *64: 64-row boxes for the dQ kernel
+  CUtensorMap tmQ, tmK, tmV, tmDO;          // 128-row boxes
+  CUtensorMap tmQ64, tmK64, tmV64, tmDO64;  // 64-row boxes (the streamed operands)
   const float* lse;    // [B, heads, nq]
   const float* delta;  // [B, heads, nq]
   __nv_bfloat16* dq;
@@ -29,477 +34,243 @@ struct AttnBwdArgs {
   float scale, scale_log2e;
 };
 
-// One query row (thread r): P and dS as bf16 into [128 rows][64 keys] SW128 tiles; rows / keys outside the problem -> zeros.
-// The same arithmetic split in two phases, so that the tensor core can compute dP of a block while the softmax warps
-// already turn its S into P (S is double-buffered in TMEM, dP is not: TMEM has 512 columns).
-// phase P: p[i] = exp2(S c - lse) for NCH chunks of 32 columns from col_begin (masked entries 0), kept in registers
-template <int NCH>
-__device__ __forceinline__ void bwd_phase_p(uint32_t t_s, int valid_keys, bool row_ok, float lse_l2, float c, int col_begin, bool full,
-                                            float (&p)[NCH * 32]) {
-  uint32_t s[NCH][32];   // all chunks are fetched before the one wait: one TMEM round trip per phase, not one per chunk
+// bf16 A-operand fragments of a 64 x 64 accumulator block (m64n64 layout -> four m64k16 register operands)
+__device__ __forceinline__ void acc_to_afrag(const float (&x)[32], uint32_t (&a)[4][4]) {
 #pragma unroll
-  for (int ch = 0; ch < NCH; ++ch) tmem_ld_32x32(t_s + col_begin + ch * 32, s[ch]);
-  tmem_ld_wait();
-#pragma unroll
-  for (int ch = 0; ch < NCH; ++ch) {
-    const int c0 = col_begin + ch * 32;
-    float xe[32];
-    scale_add32(s[ch], c, -lse_l2, xe);   // two scores per FFMA2 (the softmax warps are issue-bound)
-    if (row_ok && full) {
-#pragma unroll
-      for (int i = 0; i < 32; ++i) p[ch * 32 + i] = ex2_sel<DDPO_EXP_POLY_BWD>(i, xe[i]);
-    } else {
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const bool ok = row_ok && (c0 + i < valid_keys);
-        p[ch * 32 + i] = ok ? ex2_sel<DDPO_EXP_POLY_BWD>(i, xe[i]) : 0.f;
-      }
-    }
+  for (int kk = 0; kk < 4; ++kk) {
+    a[kk][0] = pack_bf16(x[8 * kk + 0], x[8 * kk + 1]);
+    a[kk][1] = pack_bf16(x[8 * kk + 2], x[8 * kk + 3]);
+    a[kk][2] = pack_bf16(x[8 * kk + 4], x[8 * kk + 5]);
+    a[kk][3] = pack_bf16(x[8 * kk + 6], x[8 * kk + 7]);
   }
 }
-// phase dS: ds = p (dP scale - delta scale), in place (p := ds unless KEEP_P, where ds goes to a second array)
-template <int NCH>
-__device__ __forceinline__ void bwd_phase_ds(uint32_t t_dp, float delta_s, float scale, int col_begin, const float (&p)[NCH * 32],
-                                             float (&ds)[NCH * 32]) {
-  uint32_t d[NCH][32];
+
+// bf16 store of a 64 x 64 accumulator block: rows row0 / row0 + 8 of this thread, columns 8 j + 2 (lane & 3)
+__device__ __forceinline__ void store_acc_bf16(const float (&x)[32], __nv_bfloat16* base, size_t ld, int row0, int nrows, int lane) {
 #pragma unroll
-  for (int ch = 0; ch < NCH; ++ch) tmem_ld_32x32(t_dp + col_begin + ch * 32, d[ch]);
-  tmem_ld_wait();
+  for (int h = 0; h < 2; ++h) {
+    const int row = row0 + 8 * h;
+    if (row >= nrows) continue;
+    __nv_bfloat16* o = base + static_cast<size_t>(row) * ld + 2 * (lane & 3);
 #pragma unroll
-  for (int ch = 0; ch < NCH; ++ch) {
-    float t[32];
-    scale_add32(d[ch], scale, -delta_s, t);
-#pragma unroll
-    for (int i = 0; i < 32; i += 2)
-      unpack2(mul2(pack2(p[ch * 32 + i], p[ch * 32 + i + 1]), pack2(t[i], t[i + 1])), ds[ch * 32 + i], ds[ch * 32 + i + 1]);
-  }
-}
-// bf16 store of NCH chunks of row r into [128 rows][64 keys] SW128 tiles
-template <int NCH>
-__device__ __forceinline__ void bwd_store_tile(uint8_t* sT, int r, int col_begin, const float (&v)[NCH * 32]) {
-#pragma unroll
-  for (int ch = 0; ch < NCH; ++ch) {
-    const int c0 = col_begin + ch * 32;
-    const int tile_off = (c0 >> 6) * AB_T + r * 128;
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      const int chunk = ((c0 & 63) >> 3) + g;
-      uint4 w;
-      w.x = pack_bf16(v[ch * 32 + g * 8 + 0], v[ch * 32 + g * 8 + 1]), w.y = pack_bf16(v[ch * 32 + g * 8 + 2], v[ch * 32 + g * 8 + 3]);
-      w.z = pack_bf16(v[ch * 32 + g * 8 + 4], v[ch * 32 + g * 8 + 5]), w.w = pack_bf16(v[ch * 32 + g * 8 + 6], v[ch * 32 + g * 8 + 7]);
-      *reinterpret_cast<uint4*>(sT + tile_off + ((chunk ^ (r & 7)) << 4)) = w;
-    }
+    for (int j = 0; j < 8; ++j) *reinterpret_cast<uint32_t*>(o + 8 * j) = pack_bf16(x[4 * j + 2 * h], x[4 * j + 2 * h + 1]);
   }
 }
 
 // ------------------------------------------------------------------ dK, dV ----
-// smem: K | V | 3 x (Q | dO) | P(2 tiles) | dS(2 tiles) | barriers
-//
-// Pipeline (per 128-key CTA, query blocks i = 0, 1, ...).  TMEM: S[2] (2 x 128 columns), dP (128), dV (64), dK (64) = 512.
-//   MMA lane:      S(0), dP(0), S(1); then per i: S(i+2) [as soon as the P phase of block i has read S(i)],
-//                  wait P/dS(i) -> dP(i+1), dV/dK(i)
-//   softmax warps: S(i) -> P(i) [registers]; dP(i) -> dS(i) [registers]; wait until dV/dK(i-1) have read the (P | dS) tiles;
-//                  store both
-// so the tensor core computes S(i+2) / dP(i+1) / dV, dK(i) while the softmax warps are already in the P phase of block
-// i+1 (S(i+1) has been ready for a whole block) and reaches them again before they need dP(i+1); the one (P | dS) buffer is
-// free long before the stores at the END of a block (512 MMA clocks after the previous block's hand-over), and the
-// shared memory a second buffer would take holds a third Q / dO stage instead (stage i % 3 serves S(i), dP(i), dV/dK(i):
-// with two stages the load of block i+2 could not start before dV/dK(i) had finished).  In round 1 S / dP were
-// single-buffered, the stage ring was two deep, and 28 % of the warp-stall samples sat in the two hand-over waits
-// (profiles/r2_attention.md).
+// smem: K | V (128 keys) | KV_STAGES x (Q | dO) (64 queries) | barriers
 constexpr int KV_STAGES = 3;
-constexpr int KV_SMEM_K = 0, KV_SMEM_V = AB_T, KV_SMEM_RING = 2 * AB_T, KV_SMEM_P = KV_SMEM_RING + KV_STAGES * 2 * AB_T,
-              KV_SMEM_DS = KV_SMEM_P + 2 * AB_T, KV_SMEM_BAR = KV_SMEM_DS + 2 * AB_T, KV_SMEM_TOTAL = KV_SMEM_BAR + 256;
+constexpr int KV_SMEM_K = 0, KV_SMEM_V = AB_T, KV_SMEM_RING = 2 * AB_T, KV_SMEM_BAR = KV_SMEM_RING + KV_STAGES * 2 * AB_H,
+              KV_SMEM_TOTAL = KV_SMEM_BAR + 256 + 1024;
 
 __global__ void __launch_bounds__(AB_THREADS, 1) attention_bwd_dkdv_kernel(const __grid_constant__ AttnBwdArgs p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + KV_SMEM_BAR);
   uint64_t* kv_full = bars;          // 1
-  uint64_t* qdo_full = bars + 1;     // [3]
-  uint64_t* qdo_empty = bars + 4;    // [3]
-  uint64_t* s_full = bars + 7;       // [2]
-  uint64_t* s_empty = bars + 9;      // [2] (count 8)
-  uint64_t* dp_full = bars + 11;     // 1
-  uint64_t* dp_empty = bars + 12;    // 1 (count 8)
-  uint64_t* pds_full = bars + 13;    // 1 (count 8)
-  uint64_t* pds_empty = bars + 14;   // 1
-  uint64_t* acc_full = bars + 15;    // 1
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
+  uint64_t* qdo_full = bars + 1;     // [KV_STAGES]
+  uint64_t* qdo_empty = bars + 1 + KV_STAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int k0 = blockIdx.x * 128, head = blockIdx.y, b = blockIdx.z;
-  const int nqb = (p.nq + 127) / 128;
+  const int nqb = (p.nq + 63) / 64;
 
   if (threadIdx.x == 0) {
-    if ((smem_u32(smem) & 1023u) != 0) __trap();
-    prefetch_tmap(&p.tmQ), prefetch_tmap(&p.tmK), prefetch_tmap(&p.tmV), prefetch_tmap(&p.tmDO);
     mbar_init(kv_full, 1);
-    for (int i = 0; i < KV_STAGES; ++i) mbar_init(&qdo_full[i], 1), mbar_init(&qdo_empty[i], 1);
-    for (int i = 0; i < 2; ++i) mbar_init(&s_full[i], 1), mbar_init(&s_empty[i], 8);
-    mbar_init(dp_full, 1), mbar_init(dp_empty, 8);
-    mbar_init(pds_full, 8), mbar_init(pds_empty, 1);
-    mbar_init(acc_full, 1);
+    for (int i = 0; i < KV_STAGES; ++i) mbar_init(&qdo_full[i], 1), mbar_init(&qdo_empty[i], 8);
     fence_barrier_init();
   }
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t T_S = tmem_base /* [2] x 128 */, T_DP = tmem_base + 256, T_DV = tmem_base + 384, T_DK = tmem_base + 448;
 
-  // warps 0 / 1: loops run converged, one elected lane issues TMA / MMA (operands stay in uniform registers; inside an
-  // `if (lane == 0)` region each of the 24 UMMAs per query block carried an R2UR + ELECT loop of ~20 instructions)
-  if (warp == 0) {
-    if (elect_one()) {
+  if (warp == 8) {
+    if (lane == 0) {
+      prefetch_tmap(&p.tmK), prefetch_tmap(&p.tmV), prefetch_tmap(&p.tmQ64), prefetch_tmap(&p.tmDO64);
       mbar_expect_tx(kv_full, 2 * AB_T);
       tma_load_4d(smem + KV_SMEM_K, &p.tmK, kv_full, 0, head, k0, b);
       tma_load_4d(smem + KV_SMEM_V, &p.tmV, kv_full, 0, head, k0, b);
-    }
-    __syncwarp();
-    int st = 0;
-    uint32_t ph = 0;
-    for (int i = 0; i < nqb; ++i) {
-      mbar_wait(&qdo_empty[st], ph ^ 1);
-      uint8_t* sQ = smem + KV_SMEM_RING + st * 2 * AB_T;
-      if (elect_one()) {
-        mbar_expect_tx(&qdo_full[st], 2 * AB_T);
-        tma_load_4d(sQ, &p.tmQ, &qdo_full[st], 0, head, i * 128, b);
-        tma_load_4d(sQ + AB_T, &p.tmDO, &qdo_full[st], 0, head, i * 128, b);
-      }
-      __syncwarp();
-      if (++st == KV_STAGES) st = 0, ph ^= 1;
-    }
-  } else if (warp == 1) {
-    const uint32_t id_s = umma_idesc_bf16(128, 128, 0, 0);  // S = Q K^T, dP = dO V^T
-    const uint32_t id_g = umma_idesc_bf16(128, 64, 1, 1);   // dV = P^T dO, dK = dS^T Q (both MN-major)
-    const uint32_t k_addr = smem_u32(smem + KV_SMEM_K), v_addr = smem_u32(smem + KV_SMEM_V);
-    const uint32_t p_addr = smem_u32(smem + KV_SMEM_P), ds_addr = smem_u32(smem + KV_SMEM_DS);
-    mbar_wait(kv_full, 0);
-    auto issue_s = [&](int i) {
-      const int st = i % KV_STAGES, sb = i & 1;
-      const uint32_t q_addr = smem_u32(smem + KV_SMEM_RING + st * 2 * AB_T);
-      mbar_wait(&qdo_full[st], (i / KV_STAGES) & 1);
-      mbar_wait(&s_empty[sb], ((i >> 1) & 1) ^ 1);
-      tc_fence_after();
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16(T_S + sb * 128, umma_desc(q_addr + k * 32, 16, 1024), umma_desc(k_addr + k * 32, 16, 1024), id_s, k != 0);
-        umma_commit(&s_full[sb]);
-      }
-      __syncwarp();
-    };
-    auto issue_dp = [&](int i) {
-      const int st = i % KV_STAGES;
-      const uint32_t do_addr = smem_u32(smem + KV_SMEM_RING + st * 2 * AB_T) + AB_T;
-      mbar_wait(&qdo_full[st], (i / KV_STAGES) & 1);
-      mbar_wait(dp_empty, (i & 1) ^ 1);
-      tc_fence_after();
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16(T_DP, umma_desc(do_addr + k * 32, 16, 1024), umma_desc(v_addr + k * 32, 16, 1024), id_s, k != 0);
-        umma_commit(dp_full);
-      }
-      __syncwarp();
-    };
-    issue_s(0);
-    issue_dp(0);
-    if (nqb > 1) issue_s(1);
-    for (int i = 0; i < nqb; ++i) {
-      const int st = i % KV_STAGES;
-      const uint32_t q_addr = smem_u32(smem + KV_SMEM_RING + st * 2 * AB_T), do_addr = q_addr + AB_T;
-      if (i + 2 < nqb) issue_s(i + 2);   // waits for the P phase of block i (S buffer i & 1), not for the whole block
-      mbar_wait(pds_full, i & 1);        // softmax warps are done with block i (and with dP(i))
-      if (i + 1 < nqb) issue_dp(i + 1);
-      tc_fence_after();
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {  // K = 128 query rows, 16 per instruction
-          umma_bf16(T_DV, umma_desc(p_addr + k * 2048, AB_T, 1024), umma_desc(do_addr + k * 2048, AB_T, 1024), id_g,
-                    (i | k) != 0);
-          umma_bf16(T_DK, umma_desc(ds_addr + k * 2048, AB_T, 1024), umma_desc(q_addr + k * 2048, AB_T, 1024), id_g,
-                    (i | k) != 0);
-        }
-        umma_commit(&qdo_empty[st]);
-        umma_commit(pds_empty);
-      }
-      __syncwarp();
-    }
-    if (elect_one()) umma_commit(acc_full);
-    __syncwarp();
-  } else {
-    const int q = warp & 3;
-    const int chalf = (warp - 2) >> 2;  // which 64 key columns of the 128-key block this warp handles
-    const int r = q * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>(q * 32) << 16;
-    const int valid_keys = min(128, p.nk - k0);
-    const size_t stat0 = (static_cast<size_t>(b) * p.heads + head) * p.nq;
-    // lse / delta of the NEXT query block are fetched a block ahead (the load sat right in front of its first use:
-    // 10 % of the stall samples)
-    float lse_n = 0.f, delta_n = 0.f;
-    if (r < p.nq) lse_n = p.lse[stat0 + r], delta_n = p.delta[stat0 + r];
-    for (int i = 0; i < nqb; ++i) {
-      const int sb = i & 1;
-      const int row = i * 128 + r;
-      const bool row_ok = row < p.nq;
-      const float lse_l2 = lse_n * 1.4426950408889634f, delta = delta_n;
-      if (row + 128 < p.nq) lse_n = p.lse[stat0 + row + 128], delta_n = p.delta[stat0 + row + 128];
-      float pr[64], ds[64];
-      mbar_wait(&s_full[sb], (i >> 1) & 1);
-      tc_fence_after();
-      bwd_phase_p<2>(T_S + sb * 128 + lane_off, valid_keys, row_ok, lse_l2, p.scale_log2e, chalf * 64, valid_keys == 128, pr);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_empty[sb]);
-      mbar_wait(dp_full, i & 1);
-      tc_fence_after();
-      bwd_phase_ds<2>(T_DP + lane_off, delta * p.scale, p.scale, chalf * 64, pr, ds);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(dp_empty);
-      mbar_wait(pds_empty, (i & 1) ^ 1);   // dV / dK of block i - 1 have read the (P | dS) tiles
-      bwd_store_tile<2>(smem + KV_SMEM_P, r, chalf * 64, pr);
-      bwd_store_tile<2>(smem + KV_SMEM_DS, r, chalf * 64, ds);
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(pds_full);
-    }
-    // epilogue: thread r <-> key row k0 + r
-    mbar_wait(acc_full, 0);
-    tc_fence_after();
-    const int key = k0 + r;
-#pragma unroll 1
-    for (int which = chalf; which < chalf + 1; ++which) {
-      __nv_bfloat16* dst = which == 0 ? p.dv : p.dk;
-      const int ld = which == 0 ? p.lddv : p.lddk;
-      const uint32_t t = (which == 0 ? T_DV : T_DK) + lane_off;
-#pragma unroll
-      for (int c0 = 0; c0 < 64; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(t + c0, v);
-        tmem_ld_wait();
-        if (key < p.nk) {
-          __nv_bfloat16* o = dst + (static_cast<size_t>(b) * p.nk + key) * ld + head * 64 + c0;
-#pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            uint4 u;
-            u.x = pack_bf16(__uint_as_float(v[j]), __uint_as_float(v[j + 1]));
-            u.y = pack_bf16(__uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-            u.z = pack_bf16(__uint_as_float(v[j + 4]), __uint_as_float(v[j + 5]));
-            u.w = pack_bf16(__uint_as_float(v[j + 6]), __uint_as_float(v[j + 7]));
-            *reinterpret_cast<uint4*>(o + j) = u;
-          }
-        }
+      int st = 0;
+      uint32_t ph = 0;
+      for (int i = 0; i < nqb; ++i) {
+        mbar_wait(&qdo_empty[st], ph ^ 1);
+        uint8_t* sQ = smem + KV_SMEM_RING + st * 2 * AB_H;
+        mbar_expect_tx(&qdo_full[st], 2 * AB_H);
+        tma_load_4d(sQ, &p.tmQ64, &qdo_full[st], 0, head, i * 64, b);
+        tma_load_4d(sQ + AB_H, &p.tmDO64, &qdo_full[st], 0, head, i * 64, b);
+        if (++st == KV_STAGES) st = 0, ph ^= 1;
       }
     }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+
+  // thread <-> key rows key0 / key0 + 8, query columns 8 j + 2 t4 + {0, 1} of the streamed block
+  const int wg = warp >> 2, t4 = lane & 3;
+  const int key0 = k0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const bool key_ok[2] = {key0 < p.nk, key0 + 8 < p.nk};
+  const size_t stat0 = (static_cast<size_t>(b) * p.heads + head) * p.nq;
+  const uint32_t k_addr = smem_u32(smem + KV_SMEM_K) + wg * (64 * 128), v_addr = smem_u32(smem + KV_SMEM_V) + wg * (64 * 128);
+  float dv[32], dk[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) dv[i] = 0.f, dk[i] = 0.f;
+  mbar_wait(kv_full, 0);
+  int st = 0;
+  uint32_t ph = 0;
+  for (int i = 0; i < nqb; ++i) {
+    // this thread's 16 query columns: log2-domain LSE and scaled delta
+    float lse_l2[16], delta_s[16];
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int q = i * 64 + 8 * j + 2 * t4 + e;
+        lse_l2[2 * j + e] = q < p.nq ? __ldg(p.lse + stat0 + q) * 1.4426950408889634f : 0.f;
+        delta_s[2 * j + e] = q < p.nq ? __ldg(p.delta + stat0 + q) * p.scale : 0.f;
+      }
+    mbar_wait(&qdo_full[st], ph);
+    const uint32_t q_addr = smem_u32(smem + KV_SMEM_RING + st * 2 * AB_H), do_addr = q_addr + AB_H;
+    float s[32], dp[32];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)  // S^T = K Q^T
+      Wgmma<64>::ss<0, 0>(s, gmma_desc(k_addr + k * 32, 16, 1024), gmma_desc(q_addr + k * 32, 16, 1024), k != 0);
+#pragma unroll
+    for (int k = 0; k < 4; ++k)  // dP^T = V dO^T
+      Wgmma<64>::ss<0, 0>(dp, gmma_desc(v_addr + k * 32, 16, 1024), gmma_desc(do_addr + k * 32, 16, 1024), k != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int x = 4 * j + 2 * h + e, col = 8 * j + 2 * t4 + e;
+          const bool ok = key_ok[h] && i * 64 + col < p.nq;
+          const float pr = ok ? ex2_sel<DDPO_EXP_POLY_BWD>(col, fmaf(s[x], p.scale_log2e, -lse_l2[2 * j + e])) : 0.f;
+          s[x] = pr;
+          dp[x] = pr * fmaf(dp[x], p.scale, -delta_s[2 * j + e]);
+        }
+    uint32_t pa[4][4], da[4][4];
+    acc_to_afrag(s, pa);
+    acc_to_afrag(dp, da);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {  // K = 64 query rows, 16 per instruction; B operands MN-major
+      Wgmma<64>::rs<1>(dv, pa[kk], gmma_desc(do_addr + kk * 2048, 8192, 1024), 1u);
+      Wgmma<64>::rs<1>(dk, da[kk], gmma_desc(q_addr + kk * 2048, 8192, 1024), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&qdo_empty[st]);
+    if (++st == KV_STAGES) st = 0, ph ^= 1;
   }
+  const size_t row_base = static_cast<size_t>(b) * p.nk;
+  store_acc_bf16(dv, p.dv + row_base * p.lddv + head * 64, p.lddv, key0, p.nk, lane);
+  store_acc_bf16(dk, p.dk + row_base * p.lddk + head * 64, p.lddk, key0, p.nk, lane);
 }
 
 // ---------------------------------------------------------------------- dQ ----
-// 64-key blocks, 256 TMEM columns and 113 KB of shared memory per CTA -> TWO CTAs per SM.
-// Same pipeline as the dK/dV kernel: S[2] (2 x 64 columns), dP (64), dQ (64) in TMEM, one dS tile, four K / V stages:
-//   MMA lane:      S(0), dP(0), S(1); then per key block j: S(j+2), wait dS(j) -> dP(j+1), dQ(j)
-//   softmax warps: S(j) -> P(j) [registers]; dP(j) -> dS(j) [registers]; wait until dQ(j-1) has read the dS tile; store
-// smem: Q | dO | 4 x (K | V) [64 keys each] | dS | barriers
+// smem: Q | dO (128 queries) | DQ_STAGES x (K | V) (64 keys) | barriers
 constexpr int DQ_BKV = 64;
-constexpr int DQ_KVT = DQ_BKV * 64 * 2;  // 8 KB
 constexpr int DQ_STAGES = 4;
-constexpr int DQ_THREADS = 320;          // warp0 TMA + TMEM alloc, warp1 MMA, warps 2..9 softmax/epilogue:
-                                         // 4 TMEM lane quarters x 2 halves of 32 key columns -> with 2 CTAs/SM four
-                                         // latency-bound softmax warps per scheduler instead of two
-constexpr int DQ_SMEM_Q = 0, DQ_SMEM_DO = AB_T, DQ_SMEM_RING = 2 * AB_T, DQ_SMEM_DS = DQ_SMEM_RING + DQ_STAGES * 2 * DQ_KVT,
-              DQ_SMEM_BAR = DQ_SMEM_DS + AB_T, DQ_SMEM_TOTAL = DQ_SMEM_BAR + 256;
+constexpr int DQ_SMEM_Q = 0, DQ_SMEM_DO = AB_T, DQ_SMEM_RING = 2 * AB_T, DQ_SMEM_BAR = DQ_SMEM_RING + DQ_STAGES * 2 * AB_H,
+              DQ_SMEM_TOTAL = DQ_SMEM_BAR + 256 + 1024;
 
-__global__ void __launch_bounds__(DQ_THREADS, 2) attention_bwd_dq_kernel(const __grid_constant__ AttnBwdArgs p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
+__global__ void __launch_bounds__(AB_THREADS, 1) attention_bwd_dq_kernel(const __grid_constant__ AttnBwdArgs p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + DQ_SMEM_BAR);
   uint64_t* q_full = bars;
-  uint64_t* kv_full = bars + 1;    // [4]
-  uint64_t* kv_empty = bars + 5;   // [4]
-  uint64_t* s_full = bars + 9;     // [2]
-  uint64_t* s_empty = bars + 11;   // [2] count 8
-  uint64_t* dp_full = bars + 13;
-  uint64_t* dp_empty = bars + 14;  // count 8
-  uint64_t* ds_full = bars + 15;   // count 8
-  uint64_t* ds_empty = bars + 16;
-  uint64_t* acc_full = bars + 17;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 18);
+  uint64_t* kv_full = bars + 1;               // [DQ_STAGES]
+  uint64_t* kv_empty = bars + 1 + DQ_STAGES;  // [DQ_STAGES]
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * 128, head = blockIdx.y, b = blockIdx.z;
   const int nkb = (p.nk + DQ_BKV - 1) / DQ_BKV;
 
   if (threadIdx.x == 0) {
-    if ((smem_u32(smem) & 1023u) != 0) __trap();
-    prefetch_tmap(&p.tmQ), prefetch_tmap(&p.tmK64), prefetch_tmap(&p.tmV64), prefetch_tmap(&p.tmDO);
     mbar_init(q_full, 1);
-    for (int i = 0; i < DQ_STAGES; ++i) mbar_init(&kv_full[i], 1), mbar_init(&kv_empty[i], 1);
-    for (int i = 0; i < 2; ++i) mbar_init(&s_full[i], 1), mbar_init(&s_empty[i], 8);
-    mbar_init(ds_full, 8), mbar_init(ds_empty, 1);
-    mbar_init(dp_full, 1), mbar_init(dp_empty, 8);
-    mbar_init(acc_full, 1);
+    for (int i = 0; i < DQ_STAGES; ++i) mbar_init(&kv_full[i], 1), mbar_init(&kv_empty[i], 8);
     fence_barrier_init();
   }
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, 256);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t T_S = tmem_base /* [2] x 64 */, T_DP = tmem_base + 128, T_DQ = tmem_base + 192;
 
-  if (warp == 0) {   // converged loops, elected issue (see the dK/dV kernel)
-    if (elect_one()) {
+  if (warp == 8) {
+    if (lane == 0) {
+      prefetch_tmap(&p.tmQ), prefetch_tmap(&p.tmDO), prefetch_tmap(&p.tmK64), prefetch_tmap(&p.tmV64);
       mbar_expect_tx(q_full, 2 * AB_T);
       tma_load_4d(smem + DQ_SMEM_Q, &p.tmQ, q_full, 0, head, q0, b);
       tma_load_4d(smem + DQ_SMEM_DO, &p.tmDO, q_full, 0, head, q0, b);
-    }
-    __syncwarp();
-    int st = 0;
-    uint32_t ph = 0;
-    for (int j = 0; j < nkb; ++j) {
-      mbar_wait(&kv_empty[st], ph ^ 1);
-      uint8_t* sK = smem + DQ_SMEM_RING + st * 2 * DQ_KVT;
-      if (elect_one()) {
-        mbar_expect_tx(&kv_full[st], 2 * DQ_KVT);
+      int st = 0;
+      uint32_t ph = 0;
+      for (int j = 0; j < nkb; ++j) {
+        mbar_wait(&kv_empty[st], ph ^ 1);
+        uint8_t* sK = smem + DQ_SMEM_RING + st * 2 * AB_H;
+        mbar_expect_tx(&kv_full[st], 2 * AB_H);
         tma_load_4d(sK, &p.tmK64, &kv_full[st], 0, head, j * DQ_BKV, b);
-        tma_load_4d(sK + DQ_KVT, &p.tmV64, &kv_full[st], 0, head, j * DQ_BKV, b);
+        tma_load_4d(sK + AB_H, &p.tmV64, &kv_full[st], 0, head, j * DQ_BKV, b);
+        if (++st == DQ_STAGES) st = 0, ph ^= 1;
       }
-      __syncwarp();
-      if (++st == DQ_STAGES) st = 0, ph ^= 1;
     }
-  } else if (warp == 1) {
-    const uint32_t id_s = umma_idesc_bf16(128, DQ_BKV, 0, 0);
-    const uint32_t id_q = umma_idesc_bf16(128, 64, 0, 1);  // dQ = dS K : A K-major, B (K) MN-major
-    const uint32_t q_addr = smem_u32(smem + DQ_SMEM_Q), do_addr = smem_u32(smem + DQ_SMEM_DO);
-    mbar_wait(q_full, 0);
-    // stage j % 4 holds K(j) for S(j) and dQ(j), V(j) for dP(j); S runs two blocks ahead of dQ, the fourth stage is the
-    // load in flight
-    auto issue_s = [&](int j) {
-      const int st = j % DQ_STAGES, sb = j & 1;
-      const uint32_t k_addr = smem_u32(smem + DQ_SMEM_RING + st * 2 * DQ_KVT);
-      mbar_wait(&kv_full[st], (j / DQ_STAGES) & 1);
-      mbar_wait(&s_empty[sb], ((j >> 1) & 1) ^ 1);
-      tc_fence_after();
-      if (elect_one()) {
+    return;
+  }
+
+  // thread <-> query rows row0 / row0 + 8, key columns 8 j + 2 t4 + {0, 1} of the streamed block
+  const int wg = warp >> 2, t4 = lane & 3;
+  const int row0 = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  bool row_ok[2];
+  float lse_l2[2], delta_s[2];
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16(T_S + sb * 64, umma_desc(q_addr + k * 32, 16, 1024), umma_desc(k_addr + k * 32, 16, 1024), id_s, k != 0);
-        umma_commit(&s_full[sb]);
-      }
-      __syncwarp();
-    };
-    auto issue_dp = [&](int j) {
-      const int st = j % DQ_STAGES;
-      const uint32_t v_addr = smem_u32(smem + DQ_SMEM_RING + st * 2 * DQ_KVT) + DQ_KVT;
-      mbar_wait(&kv_full[st], (j / DQ_STAGES) & 1);
-      mbar_wait(dp_empty, (j & 1) ^ 1);
-      tc_fence_after();
-      if (elect_one()) {
+  for (int h = 0; h < 2; ++h) {
+    const int row = row0 + 8 * h;
+    row_ok[h] = row < p.nq;
+    const size_t o = (static_cast<size_t>(b) * p.heads + head) * p.nq + row;
+    lse_l2[h] = row_ok[h] ? p.lse[o] * 1.4426950408889634f : 0.f;
+    delta_s[h] = row_ok[h] ? p.delta[o] * p.scale : 0.f;
+  }
+  const uint32_t q_addr = smem_u32(smem + DQ_SMEM_Q) + wg * (64 * 128), do_addr = smem_u32(smem + DQ_SMEM_DO) + wg * (64 * 128);
+  float dq[32];
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_bf16(T_DP, umma_desc(do_addr + k * 32, 16, 1024), umma_desc(v_addr + k * 32, 16, 1024), id_s, k != 0);
-        umma_commit(dp_full);
-      }
-      __syncwarp();
-    };
-    issue_s(0);
-    issue_dp(0);
-    if (nkb > 1) issue_s(1);
-    const uint32_t ds_addr = smem_u32(smem + DQ_SMEM_DS);
-    for (int j = 0; j < nkb; ++j) {
-      const int st = j % DQ_STAGES;
-      const uint32_t k_addr = smem_u32(smem + DQ_SMEM_RING + st * 2 * DQ_KVT);
-      if (j + 2 < nkb) issue_s(j + 2);   // waits for the P phase of block j only
-      mbar_wait(ds_full, j & 1);
-      if (j + 1 < nkb) issue_dp(j + 1);
-      tc_fence_after();
-      if (elect_one()) {
+  for (int i = 0; i < 32; ++i) dq[i] = 0.f;
+  mbar_wait(q_full, 0);
+  int st = 0;
+  uint32_t ph = 0;
+  for (int j = 0; j < nkb; ++j) {
+    mbar_wait(&kv_full[st], ph);
+    const uint32_t k_addr = smem_u32(smem + DQ_SMEM_RING + st * 2 * AB_H), v_addr = k_addr + AB_H;
+    float s[32], dp[32];
+    wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < DQ_BKV / 16; ++k)  // A = dS [128 q x 64 keys] K-major; B = K_j rows of 16 keys (MN-major)
-          umma_bf16(T_DQ, umma_desc(ds_addr + k * 32, 16, 1024), umma_desc(k_addr + k * 2048, DQ_KVT, 1024), id_q,
-                    (j | k) != 0);
-        umma_commit(&kv_empty[st]);
-        umma_commit(ds_empty);
-      }
-      __syncwarp();
-    }
-    if (elect_one()) umma_commit(acc_full);
-    __syncwarp();
-  } else {
-    const int q = warp & 3;
-    const int chalf = (warp - 2) >> 2;  // which 32 of the 64 key columns (and of the 64 dQ columns in the epilogue)
-    const int r = q * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>(q * 32) << 16;
-    const int row = q0 + r;
-    const bool row_ok = row < p.nq;
-    float lse_l2 = 0.f, delta = 0.f;
-    if (row_ok) {
-      const size_t o = (static_cast<size_t>(b) * p.heads + head) * p.nq + row;
-      lse_l2 = p.lse[o] * 1.4426950408889634f;
-      delta = p.delta[o];
-    }
-    const float delta_s = delta * p.scale;
-    for (int j = 0; j < nkb; ++j) {
-      const int sb = j & 1;
-      const int valid_keys = min(DQ_BKV, p.nk - j * DQ_BKV);
-      float pr[32], ds[32];
-      mbar_wait(&s_full[sb], (j >> 1) & 1);
-      tc_fence_after();
-      bwd_phase_p<1>(T_S + sb * 64 + lane_off, valid_keys, row_ok, lse_l2, p.scale_log2e, chalf * 32, valid_keys == DQ_BKV, pr);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_empty[sb]);
-      mbar_wait(dp_full, j & 1);
-      tc_fence_after();
-      bwd_phase_ds<1>(T_DP + lane_off, delta_s, p.scale, chalf * 32, pr, ds);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(dp_empty);
-      mbar_wait(ds_empty, (j & 1) ^ 1);   // dQ of block j - 1 has read the dS tile
-      bwd_store_tile<1>(smem + DQ_SMEM_DS, r, chalf * 32, ds);
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(ds_full);
-    }
-    mbar_wait(acc_full, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int c0 = chalf * 32; c0 < chalf * 32 + 32; c0 += 32) {
-      uint32_t v[32];
-      tmem_ld_32x32(T_DQ + lane_off + c0, v);
-      tmem_ld_wait();
-      if (row_ok) {
-        __nv_bfloat16* o = p.dq + (static_cast<size_t>(b) * p.nq + row) * p.lddq + head * 64 + c0;
+    for (int k = 0; k < 4; ++k)  // S = Q K^T
+      Wgmma<64>::ss<0, 0>(s, gmma_desc(q_addr + k * 32, 16, 1024), gmma_desc(k_addr + k * 32, 16, 1024), k != 0);
 #pragma unroll
-        for (int j = 0; j < 32; j += 8) {
-          uint4 u;
-          u.x = pack_bf16(__uint_as_float(v[j]), __uint_as_float(v[j + 1]));
-          u.y = pack_bf16(__uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-          u.z = pack_bf16(__uint_as_float(v[j + 4]), __uint_as_float(v[j + 5]));
-          u.w = pack_bf16(__uint_as_float(v[j + 6]), __uint_as_float(v[j + 7]));
-          *reinterpret_cast<uint4*>(o + j) = u;
+    for (int k = 0; k < 4; ++k)  // dP = dO V^T
+      Wgmma<64>::ss<0, 0>(dp, gmma_desc(do_addr + k * 32, 16, 1024), gmma_desc(v_addr + k * 32, 16, 1024), k != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    const int valid_keys = p.nk - j * DQ_BKV;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int x = 4 * jj + 2 * h + e, col = 8 * jj + 2 * t4 + e;
+          const bool ok = row_ok[h] && col < valid_keys;
+          const float pr = ok ? ex2_sel<DDPO_EXP_POLY_BWD>(col, fmaf(s[x], p.scale_log2e, -lse_l2[h])) : 0.f;
+          dp[x] = pr * fmaf(dp[x], p.scale, -delta_s[h]);
         }
-      }
-    }
+    uint32_t da[4][4];
+    acc_to_afrag(dp, da);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)  // dQ += dS K: B = K rows of 16 keys (MN-major)
+      Wgmma<64>::rs<1>(dq, da[kk], gmma_desc(k_addr + kk * 2048, 8192, 1024), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&kv_empty[st]);
+    if (++st == DQ_STAGES) st = 0, ph ^= 1;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
-  }
+  store_acc_bf16(dq, p.dq + static_cast<size_t>(b) * p.nq * p.lddq + head * 64, p.lddq, row0, p.nq, lane);
 }
 
 // delta[b,h,q] = sum_d dO * O ; 8 threads per (row, head), 16-byte loads
@@ -554,8 +325,10 @@ extern "C" int ddpo_attention_bwd(const ddpo_attention_bwd_args* a, void* stream
   if ((rc = make_map(&p.tmK, a->k, a->heads, a->nk, a->batch, a->ldk))) return rc;
   if ((rc = make_map(&p.tmV, a->v, a->heads, a->nk, a->batch, a->ldv))) return rc;
   if ((rc = make_map(&p.tmDO, a->dout, a->heads, a->nq, a->batch, a->lddo))) return rc;
-  if ((rc = make_map(&p.tmK64, a->k, a->heads, a->nk, a->batch, a->ldk, DQ_BKV))) return rc;
-  if ((rc = make_map(&p.tmV64, a->v, a->heads, a->nk, a->batch, a->ldv, DQ_BKV))) return rc;
+  if ((rc = make_map(&p.tmQ64, a->q, a->heads, a->nq, a->batch, a->ldq, 64))) return rc;
+  if ((rc = make_map(&p.tmK64, a->k, a->heads, a->nk, a->batch, a->ldk, 64))) return rc;
+  if ((rc = make_map(&p.tmV64, a->v, a->heads, a->nk, a->batch, a->ldv, 64))) return rc;
+  if ((rc = make_map(&p.tmDO64, a->dout, a->heads, a->nq, a->batch, a->lddo, 64))) return rc;
   p.lse = a->lse, p.delta = a->delta;
   p.dq = static_cast<__nv_bfloat16*>(a->dq), p.dk = static_cast<__nv_bfloat16*>(a->dk);
   p.dv = static_cast<__nv_bfloat16*>(a->dv);
@@ -577,7 +350,7 @@ extern "C" int ddpo_attention_bwd(const ddpo_attention_bwd_args* a, void* stream
   attention_bwd_dkdv_kernel<<<g1, AB_THREADS, KV_SMEM_TOTAL, stream>>>(p);
   DDPO_LAUNCH_OK();
   dim3 g2((a->nq + 127) / 128, a->heads, a->batch);
-  attention_bwd_dq_kernel<<<g2, DQ_THREADS, DQ_SMEM_TOTAL, stream>>>(p);
+  attention_bwd_dq_kernel<<<g2, AB_THREADS, DQ_SMEM_TOTAL, stream>>>(p);
   DDPO_LAUNCH_OK();
   return DDPO_OK;
 }

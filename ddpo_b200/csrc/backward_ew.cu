@@ -333,7 +333,7 @@ __global__ void gather_rows_kernel(const float* __restrict__ src, const int64_t*
 
 static inline int grid_for(int64_t n, int threads) {
   int64_t g = (n + threads - 1) / threads;
-  const int64_t cap = 148 * 32;
+  const int64_t cap = 132 * 32;
   return static_cast<int>(g > cap ? cap : (g < 1 ? 1 : g));
 }
 

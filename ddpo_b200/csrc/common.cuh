@@ -1,6 +1,6 @@
-// Shared device/host helpers for libddpo_b200 (sm_100a only).
-// PTX wrappers for mbarrier, TMA (cp.async.bulk.tensor) and tcgen05 (alloc / mma /
-// commit / ld), UMMA shared-memory + instruction descriptors, status handling.
+// Shared device/host helpers for libddpo_b200 (sm_90a only).
+// PTX wrappers for mbarrier, TMA (cp.async.bulk.tensor) and wgmma (fence / commit / wait,
+// shared-memory matrix descriptors), status handling.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -43,41 +43,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.b32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-// packed fp32 pairs (sm_100: FFMA2 / FMUL2 execute two lanes' worth of fp32 in one issue slot; each half is an ordinary
-// round-to-nearest fma / mul, so results are bit-identical to the scalar instructions) -- the softmax warps of the
-// attention kernels are issue-bound
-__device__ __forceinline__ uint64_t pack2(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack2(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t mul2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-// x[i] = x[i] * b + c for 32 values held as 32-bit registers (pairs are consecutive registers)
-__device__ __forceinline__ void scale_add32(uint32_t (&v)[32], float b, float c, float (&out)[32]) {
-  const uint64_t b2 = pack2(b, b), c2 = pack2(c, c);
-#pragma unroll
-  for (int i = 0; i < 32; i += 2)
-    unpack2(fma2(pack2(__uint_as_float(v[i]), __uint_as_float(v[i + 1])), b2, c2), out[i], out[i + 1]);
-}
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -154,9 +119,8 @@ __device__ __forceinline__ float ex2_poly(float x) {
 
 // Which columns of a 32-wide chunk take the polynomial: every DDPO_EXP_POLY_{FWD,BWD}-th one (0 = none).  The split
 // is a fixed function of the element's position, so results stay deterministic and batch invariant.
-// Measured on B200 (64x64 self-attention, batch 40, us fwd / bwd): period 2: 1664 / 5699, 4: 1501 / 5541,
-// 8: 1485 / 5457, none: 1539 / 5392 -- the polynomial costs ~10 issue slots against 1 for MUFU.EX2 and the softmax
-// warps are issue bound, so only the forward kernel (fewer other instructions per score) keeps a small share.
+// The polynomial costs ~10 issue slots against 1 for MUFU.EX2, so only the forward kernel (fewer other instructions
+// per score) keeps a small share.
 #ifndef DDPO_EXP_POLY_FWD
 #define DDPO_EXP_POLY_FWD 8
 #endif
@@ -199,8 +163,8 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 }
 // Bounded wait: a protocol bug traps (reported as a CUDA error) instead of hanging the GPU.
 // try_wait already suspends the warp for a hardware-chosen interval; the clock is read once every 256 retries so the
-// retry loop stays at 3 instructions.  (A long explicit suspend-time hint was measured: no gain for the attention
-// kernels, -3 % on the large GEMMs whose MMA/TMA threads then wake up late.)
+// retry loop stays at 3 instructions.  No explicit suspend-time hint: a waiting producer or consumer should wake up as
+// soon as its barrier completes.
 #ifndef DDPO_MBAR_TIMEOUT_CYCLES
 #define DDPO_MBAR_TIMEOUT_CYCLES 8000000000ll  // ~4 s at 2 GHz
 #endif
@@ -274,135 +238,28 @@ __device__ __forceinline__ void bulk_wait_read() {  // all but the N most recent
 }
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ---------------------------------------------------------------- tcgen05 ----
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem], bf16 inputs, fp32 accumulate, cta_group::1
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 columns of 32-bit: thread i of the warp gets lane (base_lane+i), columns c..c+31
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ----------------------------------------------------- CTA-pair (cta_group::2) ----
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// In a CTA pair the shared::cluster address of the SAME offset in the even (leader) CTA is obtained by clearing
-// bit 24 of the local shared address (CUTLASS Sm100MmaPeerBitMask).
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-// TMA loads of a CTA pair: data lands in the issuing CTA's shared memory, completion bytes are credited to the
-// LEADER CTA's mbarrier (only the leader issues the MMAs).
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
-                                                int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-      "%6}], [%2];" ::"r"(smem_u32(smem_dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-// D[tmem of both CTAs] (+)= A[smem of both CTAs, 128 rows each] * B[smem of both CTAs, N/2 rows each]; leader only
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (once all previously issued MMAs completed) on the mbarrier at the same offset in the CTAs of `mask`
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(mask)
-               : "memory");
-}
-// arrive on the mbarrier at the same offset in CTA `cta` of the cluster.  RELAXED: the only data the waiter depends on
-// are TMEM reads, ordered by tcgen05.fence::before_thread_sync; a .release.cluster arrive compiles to
-// MEMBAR.ALL.GPU + ERRBAR and stalls the epilogue warp until all of its global stores are acknowledged
-// (16 % of the stall samples of the GEGLU linear, profiles/r1_linear_epilogue.md).
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [ra];\n\t}\n" ::"r"(smem_u32(bar)),
-      "r"(cta)
-      : "memory");
-}
-
-// UMMA shared-memory matrix descriptor (sm_100: version=1 at bit 46, layout type at [61,64)).
-// SWIZZLE_128B = 2.  Addresses/offsets are encoded >>4.
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// ------------------------------------------------------------------ wgmma ----
+// Shared-memory matrix descriptor of a SWIZZLE_128B operand (sm_90): start address, leading and stride byte offsets
+// (all >> 4), layout type 1 = 128-byte swizzle at bits [62, 64).  K-major tiles are rows of 64 bf16 (128 B) in 8-row
+// atoms of 1 KB: SBO = 1024, LBO unused.  MN-major tiles: LBO = distance between 64-element MN blocks, SBO = distance
+// between 8-row K groups.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;  // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;  // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;  // SWIZZLE_128B
   return d;
 }
-// Instruction descriptor for kind::f16 with BF16 A/B, FP32 D.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4)                                  // D format F32
-         | (1u << 7)                                // A format BF16
-         | (1u << 10)                               // B format BF16
-         | (static_cast<uint32_t>(a_mn_major) << 15)  // A major (0 = K)
-         | (static_cast<uint32_t>(b_mn_major) << 16)  // B major (0 = K)
-         | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// barrier among `count` threads (a multiple of 32) on hardware barrier `id` (id 0 is __syncthreads)
+__device__ __forceinline__ void named_barrier(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
 #endif  // __CUDACC__
 

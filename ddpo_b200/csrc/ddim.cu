@@ -240,7 +240,7 @@ extern "C" int ddpo_threefry_normal(const uint32_t* key_dev, float* out, int64_t
   DDPO_REQUIRE(n > 0 && n < (int64_t(1) << 32), "ddpo_threefry_normal: n out of range");
   const int threads = 256;
   int64_t blocks = ((n + 1) / 2 + threads - 1) / threads;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   threefry_normal_kernel<<<(int)blocks, threads, 0, static_cast<cudaStream_t>(stream)>>>(key_dev, out, (uint32_t)n);
   DDPO_LAUNCH_OK();
   return DDPO_OK;

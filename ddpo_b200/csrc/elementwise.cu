@@ -357,7 +357,7 @@ __global__ void __launch_bounds__(DS_WARPS * 32) dense_small_grouped_kernel(cons
 
 static inline int grid_for(int64_t n, int threads) {
   int64_t g = (n + threads - 1) / threads;
-  const int64_t cap = 148 * 32;
+  const int64_t cap = 132 * 32;
   return static_cast<int>(g > cap ? cap : (g < 1 ? 1 : g));
 }
 

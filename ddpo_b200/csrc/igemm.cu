@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution / linear layer on tcgen05 (sm_100a).
+// Implicit-GEMM convolution / linear layer on wgmma (sm_90a).
 //
 //   out[m, n] = epilogue( sum_{tap, c} A[(b, y*s+dy-p, x*s+dx-p), c] * Wt[n, (tap, c)] )
 //
@@ -6,245 +6,276 @@
 // `unet.apply` (reference call sites: pipeline_flax_stable_diffusion.py:219-224,
 // training/policy_gradient.py:87-102): nn.Conv 3x3 / 3x3 stride-2 / 1x1 and nn.Dense.
 //
-// Design (B200-first, not a translation of anything):
-//  * persistent kernel, one CTA per SM, static round-robin tile scheduler (n fastest so
-//    the 128-row activation tile is re-used out of L2 by consecutive CTAs);
-//  * warp 0 = TMA producer.  The activation operand is fetched straight from the NHWC
-//    bf16 tensor with a 4-D tiled tensor map whose box is (64 ch, bw, bh, bb) pixels;
-//    the 3x3 taps are the same box shifted by (dx-1, dy-1) and TMA's out-of-bounds
-//    zero fill IS the conv padding -> no im2col buffer ever exists.  Channel-concatenated
-//    inputs (U-Net skip connections) are two tensor maps walked back to back;
-//  * warp 1 = single-thread tcgen05.mma issuer, 128 x BN x 16 bf16 UMMAs, fp32
-//    accumulators in TMEM, double-buffered (2 x 256 columns) so the epilogue of tile i
-//    overlaps the main loop of tile i+1;
-//  * warps 4..11 = epilogue (two warps per TMEM lane quarter, alternating 32-column chunks):
-//    tcgen05.ld 32x32b, fused bias / per-sample time-embedding
-//    row vector / fp32 residual / GEGLU, 128-bit stores;
-//  * K order is fixed and independent of the batch size and of the position of a row in
-//    its tile -> results are batch-invariant and bit-reproducible (the PPO ratio of an
-//    unchanged policy must be exactly 1; reference config/base.py:88 clip 1e-4).
-#include "igemm_common.cuh"
+// Design:
+//  * one CTA per 128 x BN output tile (n fastest, so the 128-row activation tile of consecutive CTAs is re-used out
+//    of L2); BN is a template parameter because it is the N of the wgmma instruction;
+//  * warp 8 = TMA producer.  The activation operand is fetched straight from the NHWC bf16 tensor with a 4-D tiled
+//    tensor map whose box is (64 ch, bw, bh, bb) pixels; the 3x3 taps are the same box shifted by (dx-1, dy-1) and
+//    TMA's out-of-bounds zero fill IS the conv padding -> no im2col buffer ever exists.  Channel-concatenated inputs
+//    (U-Net skip connections) are two tensor maps walked back to back.  Stages of a multi-stage ring are handed over
+//    through full / empty mbarriers;
+//  * warps 0-7 = two consumer warpgroups, 64 rows each: m64nBNk16 bf16 wgmma from shared memory (both operands
+//    K-major, 128-byte swizzle), fp32 accumulators in registers, one k-block of wgmma in flight while the next is
+//    issued;
+//  * epilogue: the accumulators go through shared memory (the drained stage ring) so that every global access of the
+//    fused bias / per-sample time-embedding row vector / fp32 residual / GEGLU / slab statistics is coalesced;
+//  * K order is fixed and independent of the batch size, of the tile width and of the position of a row in its
+//    tile -> results are batch-invariant and bit-reproducible (the PPO ratio of an unchanged policy must be exactly 1;
+//    reference config/base.py:88 clip 1e-4).
+#include "common.cuh"
+#include "wgmma.cuh"
 
 namespace ddpo {
 
-__global__ void __launch_bounds__(IGEMM_THREADS, 1) igemm_kernel(const __grid_constant__ IGemmArgs p) {
+constexpr int BM = 128;
+constexpr int BK = 64;
+constexpr int A_TILE_BYTES = BM * BK * 2;
+constexpr int IGEMM_THREADS = 288;  // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int IGEMM_CONSUMERS = 256;
+constexpr int SMEM_BUDGET = 227 * 1024 - 1024 /*align slack*/ - 256 /*barriers*/;
+
+struct IGemmArgs {
+  CUtensorMap tmA0, tmA1, tmB;
+  int M_total, N_total, stages;
+  int taps, kc0, kc1;
+  int is_conv, W, H, conv_stride, pad;
+  const float* bias;      // [N] or null
+  const float* rowvec;    // [B, rowvec_ld] or null: added per sample (time-embedding projection)
+  int rows_per_sample, rowvec_ld;
+  const float* residual;  // [M, ld_res] fp32 or null
+  int ld_res;
+  float* out_f32;         // [M, ld_out] or null
+  __nv_bfloat16* out_bf16;  // [M, ld_out] or null  (GEGLU: [M, ld_out] with N/2 useful columns)
+  int ld_out;
+  int geglu;
+  int accumulate_out;     // out_f32 += result (used by backward passes that sum two branches)
+  float* gn_stats;        // [ceil(M/32), N, 2] or null: per 32-row slab, per column (sum, sum of squares) of the fp32 OUTPUT
+                          // values -- the GroupNorm that consumes out_f32 takes its statistics from these instead of
+                          // re-reading the tensor (norm.cu gn_finalize_kernel)
+  __nv_bfloat16* aux_bf16;  // GEGLU only: pre-activation [M, N] (tile-interleaved, bias included) kept for backward
+};
+
+template <int BN>
+constexpr int igemm_stage_bytes() { return A_TILE_BYTES + BN * BK * 2; }
+template <int BN>
+constexpr int igemm_epi_bytes() { return BM * (BN + 4) * 4; }  // fp32 tile, rows padded by 16 B against bank conflicts
+
+__device__ __forceinline__ float4 add4(float4 a, float4 b) { return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
+__device__ __forceinline__ uint2 pack_bf16x4(float4 v) { return make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w)); }
+
+template <int BN>
+__global__ void __launch_bounds__(IGEMM_THREADS, BN <= 128 ? 2 : 1) igemm_kernel(const __grid_constant__ IGemmArgs p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int BN = p.BN;
+  constexpr int SB = igemm_stage_bytes<BN>();
+  constexpr int EPI = igemm_epi_bytes<BN>();
   const int stages = p.stages;
-  const int b_tile_bytes = BN * BK * 2;
-  const int MT = p.MT;
-  const int a_bytes = MT * A_TILE_BYTES;
-  const int stage_bytes = a_bytes + b_tile_bytes;
-  const int nbuf = MT == 2 ? 1 : 2;  // MT = 2 uses all 512 TMEM columns for one tile (no accumulator double buffering)
-  uint8_t* epi_base = smem;  // [EPI_STAGE_BYTES] of the coalescing register epilogue
-  if (p.epi_stage) smem += EPI_STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + stages * stage_bytes);
+  const int main_bytes = stages * SB > EPI ? stages * SB : EPI;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + main_bytes);
   uint64_t* empty_bar = full_bar + stages;
-  uint64_t* tmem_full = empty_bar + stages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  const int TM = BM * MT;
-  const int tiles_m = (p.M_total + TM - 1) / TM;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles_n = p.N_total / BN;
-  const int num_tiles = tiles_m * tiles_n;
+  const int tm = blockIdx.x / tiles_n, tn = blockIdx.x % tiles_n;
+  const int m0 = tm * BM, n0 = tn * BN;
   const int kcs = p.kc0 + p.kc1;
   const int kiters = p.taps * kcs;
 
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&p.tmA0);
-    prefetch_tmap(&p.tmA1);
-    prefetch_tmap(&p.tmB);
-  }
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int i = 0; i < stages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 8);
+      mbar_init(&empty_bar[i], IGEMM_CONSUMERS / 32);
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // single-role warps: loops run converged, one elected lane issues (operands in uniform registers; see igemm2.cu)
-  if (warp == 0) {
+  if (warp == 8) {
     // ------------------------------------------------------------ TMA producer
-    int stage = 0;
-    uint32_t phase = 0;
-    const int HW = p.W * p.H;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int tm = tile / tiles_n, tn = tile % tiles_n;
-      const int m0 = tm * TM, n0 = tn * BN;
+    if (lane == 0) {
+      prefetch_tmap(&p.tmA0);
+      prefetch_tmap(&p.tmA1);
+      prefetch_tmap(&p.tmB);
+      int b0 = 0, h0 = 0, w0 = 0;
+      if (p.is_conv) {
+        const int HW = p.W * p.H;
+        b0 = m0 / HW;
+        h0 = (m0 % HW) / p.W;
+        w0 = m0 % p.W;  // non-zero only when a pixel row is wider than a tile (W > 128)
+      }
+      int stage = 0;
+      uint32_t phase = 0;
       int kit = 0;
       for (int tap = 0; tap < p.taps; ++tap) {
         const int dy = p.taps == 9 ? tap / 3 : 0, dx = p.taps == 9 ? tap - dy * 3 : 0;
         for (int ch = 0; ch < kcs; ++ch, ++kit) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sA = smem + stage * stage_bytes;
-          uint8_t* sB = sA + a_bytes;
-          if (elect_one()) {
-            mbar_expect_tx(&full_bar[stage], stage_bytes);
-            for (int sub = 0; sub < MT; ++sub) {
-              const int ms = m0 + sub * BM;
-              if (p.is_conv) {
-                const int b0 = ms / HW, h0 = (ms % HW) / p.W;
-                const int w0 = ms % p.W;  // non-zero only when a pixel row is wider than a tile (W > 128)
-                const int cx = w0 * p.conv_stride + dx - p.pad;
-                const int cy = h0 * p.conv_stride + dy - p.pad;
-                if (ch < p.kc0)
-                  tma_load_4d(sA + sub * A_TILE_BYTES, &p.tmA0, &full_bar[stage], ch * BK, cx, cy, b0);
-                else
-                  tma_load_4d(sA + sub * A_TILE_BYTES, &p.tmA1, &full_bar[stage], (ch - p.kc0) * BK, cx, cy, b0);
-              } else {
-                tma_load_2d(sA + sub * A_TILE_BYTES, &p.tmA0, &full_bar[stage], kit * BK, ms);
-              }
-            }
-            tma_load_2d(sB, &p.tmB, &full_bar[stage], kit * BK, n0);
+          uint8_t* sA = smem + stage * SB;
+          mbar_expect_tx(&full_bar[stage], SB);
+          if (p.is_conv) {
+            const int cx = w0 * p.conv_stride + dx - p.pad;
+            const int cy = h0 * p.conv_stride + dy - p.pad;
+            if (ch < p.kc0)
+              tma_load_4d(sA, &p.tmA0, &full_bar[stage], ch * BK, cx, cy, b0);
+            else
+              tma_load_4d(sA, &p.tmA1, &full_bar[stage], (ch - p.kc0) * BK, cx, cy, b0);
+          } else {
+            tma_load_2d(sA, &p.tmA0, &full_bar[stage], kit * BK, m0);
           }
-          __syncwarp();
-          if (++stage == stages) {
-            stage = 0;
-            phase ^= 1;
-          }
+          tma_load_2d(sA + A_TILE_BYTES, &p.tmB, &full_bar[stage], kit * BK, n0);
+          if (++stage == stages) stage = 0, phase ^= 1;
         }
       }
     }
-  } else if (warp == 1) {
-    // -------------------------------------------------------------- MMA issuer
-    const uint32_t idesc = umma_idesc_bf16(BM, BN, 0, 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int buf = it % nbuf;
-      mbar_wait(&tmem_empty[buf], ((it / nbuf) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + buf * 256;
-      for (int kit = 0; kit < kiters; ++kit) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t a_base = smem_u32(smem + stage * stage_bytes);
-        const uint32_t b_base = a_base + a_bytes;
-        if (elect_one()) {
-          for (int sub = 0; sub < MT; ++sub) {
-#pragma unroll
-            for (int k = 0; k < BK / 16; ++k) {
-              umma_bf16(d_tmem + sub * 256, umma_desc(a_base + sub * A_TILE_BYTES + k * 32, 16, 1024),
-                        umma_desc(b_base + k * 32, 16, 1024), idesc, (kit | k) != 0);
-            }
-          }
-          umma_commit(&empty_bar[stage]);
-        }
-        __syncwarp();
-        if (++stage == stages) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      if (elect_one()) umma_commit(&tmem_full[buf]);
-      __syncwarp();
-    }
-  } else if (warp >= 4) {
-    // ---------------------------------------------------------------- epilogue
-    const int q = warp & 3;
-    const int wgrp = (warp - 4) >> 2;
-    // MT = 1: the two warps of a lane quarter alternate 32-column chunks; MT = 2: one warp group per 128-row sub-tile
-    const int cgrp = MT == 2 ? 0 : wgrp;
-    const int cstep = MT == 2 ? 32 : 64;
-    const int sub = MT == 2 ? wgrp : 0;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int tm = tile / tiles_n, tn = tile % tiles_n;
-      const int m0 = tm * TM + sub * BM, n0 = tn * BN;
-      const int buf = it % nbuf;
-      mbar_wait(&tmem_full[buf], (it / nbuf) & 1);
-      tc_fence_after();
-      const int row = m0 + q * 32 + lane;
-      const bool row_ok = row < p.M_total;
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + buf * 256 + sub * 256;
-      if (p.epi_stage) {
-        igemm_epilogue_staged(p, epi_base + (warp - 4) * EPI_STAGE_WARP_BYTES, t_row, m0 + q * 32, lane, n0, BN, cgrp, cstep, [&]() {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty[buf]);
-        });
-      } else {
-        igemm_epilogue(p, t_row, row, row_ok, n0, tn, BN, cgrp, cstep);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty[buf]);
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  // -------------------------------------------------------------- consumers
+  const int wg = warp >> 2;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  {
+    int stage = 0, prev = 0;
+    uint32_t phase = 0;
+    for (int kit = 0; kit < kiters; ++kit) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t a_base = smem_u32(smem + stage * SB) + wg * (64 * 128);
+      const uint32_t b_base = smem_u32(smem + stage * SB + A_TILE_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k)
+        Wgmma<BN>::template ss<0, 0>(acc, gmma_desc(a_base + k * 32, 16, 1024), gmma_desc(b_base + k * 32, 16, 1024),
+                                     (kit | k) != 0);
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous k-block has finished reading its stage
+      if (kit > 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == stages) stage = 0, phase ^= 1;
+    }
+    wgmma_wait<0>();
+  }
+  named_barrier(1, IGEMM_CONSUMERS);  // every operand stage has been read: the ring becomes the epilogue tile
+
+  // ---------------------------------------------------------------- epilogue
+  constexpr int P = BN + 4;
+  float* stg = reinterpret_cast<float*>(smem);
+  {
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      *reinterpret_cast<float2*>(stg + r0 * P + 8 * j + cq) = make_float2(acc[4 * j], acc[4 * j + 1]);
+      *reinterpret_cast<float2*>(stg + (r0 + 8) * P + 8 * j + cq) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+    }
+  }
+  named_barrier(1, IGEMM_CONSUMERS);
+  const int tid = threadIdx.x;
+  if (p.geglu) {
+    // GEGLU: this N tile is [BN/2 linear | BN/2 gate] columns of the same output channels (host-side row permutation):
+    // out = lin * gelu_tanh(gate) -> out_bf16[:, tn*BN/2 + c], pre-activations (training) -> aux[:, n0 + c] / [n0 + BN/2 + c]
+    constexpr int HALF = BN / 2, H4 = HALF / 4;
+    for (int idx = tid; idx < BM * H4; idx += IGEMM_CONSUMERS) {
+      const int r = idx / H4, c = (idx % H4) * 4;
+      const int row = m0 + r;
+      if (row >= p.M_total) continue;
+      const int n = n0 + c;
+      const float4 lin = add4(*reinterpret_cast<const float4*>(stg + r * P + c), __ldg(reinterpret_cast<const float4*>(p.bias + n)));
+      const float4 gate =
+          add4(*reinterpret_cast<const float4*>(stg + r * P + HALF + c), __ldg(reinterpret_cast<const float4*>(p.bias + n + HALF)));
+      const float4 f = make_float4(lin.x * gelu_tanh_f(gate.x), lin.y * gelu_tanh_f(gate.y), lin.z * gelu_tanh_f(gate.z),
+                                   lin.w * gelu_tanh_f(gate.w));
+      *reinterpret_cast<uint2*>(p.out_bf16 + static_cast<size_t>(row) * p.ld_out + tn * HALF + c) = pack_bf16x4(f);
+      if (p.aux_bf16 != nullptr) {
+        __nv_bfloat16* ax = p.aux_bf16 + static_cast<size_t>(row) * p.N_total + n;
+        *reinterpret_cast<uint2*>(ax) = pack_bf16x4(lin);
+        *reinterpret_cast<uint2*>(ax + HALF) = pack_bf16x4(gate);
+      }
+    }
+    return;
+  }
+  constexpr int C4 = BN / 4;
+  for (int idx = tid; idx < BM * C4; idx += IGEMM_CONSUMERS) {
+    const int r = idx / C4, c = (idx % C4) * 4;
+    const int row = m0 + r;
+    float4 f = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (row < p.M_total) {
+      const int n = n0 + c;
+      f = *reinterpret_cast<const float4*>(stg + r * P + c);
+      if (p.bias != nullptr) f = add4(f, __ldg(reinterpret_cast<const float4*>(p.bias + n)));
+      if (p.rowvec != nullptr)
+        f = add4(f, __ldg(reinterpret_cast<const float4*>(p.rowvec + static_cast<size_t>(row / p.rows_per_sample) * p.rowvec_ld + n)));
+      if (p.residual != nullptr) f = add4(f, *reinterpret_cast<const float4*>(p.residual + static_cast<size_t>(row) * p.ld_res + n));
+      if (p.out_f32 != nullptr) {
+        float4* o = reinterpret_cast<float4*>(p.out_f32 + static_cast<size_t>(row) * p.ld_out + n);
+        if (p.accumulate_out) f = add4(f, *o);
+        *o = f;
+      }
+      if (p.out_bf16 != nullptr)
+        *reinterpret_cast<uint2*>(p.out_bf16 + static_cast<size_t>(row) * p.ld_out + n) = pack_bf16x4(f);
+    }
+    if (p.gn_stats != nullptr) *reinterpret_cast<float4*>(stg + r * P + c) = f;  // rows outside the matrix count as zeros
+  }
+  if (p.gn_stats == nullptr) return;
+  named_barrier(1, IGEMM_CONSUMERS);
+  // slab statistics: per 32-row slab and column, (sum, sum of squares) over the rows in order -- a function of the 32
+  // values only
+  for (int idx = tid; idx < (BM / 32) * BN; idx += IGEMM_CONSUMERS) {
+    const int s = idx / BN, c = idx % BN;
+    const int m_slab = m0 + s * 32;
+    if (m_slab >= p.M_total) continue;
+    float sum = 0.f, sq = 0.f;
+#pragma unroll 8
+    for (int r = 0; r < 32; ++r) {
+      const float v = stg[(s * 32 + r) * P + c];
+      sum += v;
+      sq = fmaf(v, v, sq);
+    }
+    *reinterpret_cast<float2*>(p.gn_stats + (static_cast<size_t>(m_slab >> 5) * p.N_total + n0 + c) * 2) = make_float2(sum, sq);
   }
 }
 
-// Width of the CTA(-pair) tile: BN = UMMA N (multiple of 32, <= 256, divides N; GEGLU needs BN/2 % 32 == 0), or -- CTA
-// pairs only -- 320 = two 160-column sub-tiles that share ONE fetch of the activation tile (igemm2.cu, NS = 2).  Tile
-// shape is a pure scheduling choice (the K order of every output element is fixed), so it is picked by a cost model:
-//   time ~ waves x (k-blocks x clks per k-block + fixed tile overhead)
-// with, per 64-deep k-block and per SM,
-//   * the tensor pipe: 2 * width clks (4096 MAC/clk/SM);
-//   * operand delivery: every tap and every column tile re-reads its operands out of L2, and what a CTA's producer warps
-//     get into shared memory per clock is bounded in practice (TMA issue + L2 round trips; 32-40 B/clk/SM observed in
-//     every long-K launch, 64-76 B/clk/SM in a pure pull loop: tests/microbench/l2_tma_bw.cu, profiles/r2_igemm.md).  The
-//     model charges 16 KB of activations + 64 B x width of weights per CTA of a pair (128 B x width for a single CTA)
-//     at 35 B/clk: an empirical constant that ranks the tilings the way the measurements do -- wider tiles = fewer
-//     operand bytes per FLOP;
-//   * the shared-memory port (128 B/clk: TMA writes + MMA reads; the activation tile is read once per sub-tile).
-// Narrower tiles win only when the widest tiling leaves most SMs idle in the last wave (e.g. 80 tiles on 74 pairs).
-static int pick_width(int N, int geglu, int M_total, int kiters, bool pair, bool allow_wide) {
-  const int step = geglu ? 64 : 32;
-  const int workers = pair ? num_sms() / 2 : num_sms();
-  const int rows = pair ? 2 * BM : BM;
-  const long tiles_m = (M_total + rows - 1) / rows;
-  int best = 0;
-  long best_cost = 0;
-  for (int w = (pair && allow_wide && !geglu) ? 320 : 256; w >= step; w -= step) {
-    if (w > 256 && w != 320) continue;
-    if (N % w != 0) continue;
-    const int ns = w > 256 ? 2 : 1;
-    const long tiles = tiles_m * (N / w);
-    const long waves = (tiles + workers - 1) / workers;
-    const long mma = 2L * w;
-    const long bytes = 16384L + (pair ? 64L : 128L) * w;
-    const long l2 = bytes / 35;
-    const long port = 128L + 128L * ns + (pair ? 1L : 2L) * w;
-    long kb = mma > l2 ? mma : l2;
-    if (port > kb) kb = port;
-    // fixed cost per tile: pipeline hand-over; the wide tile cannot double-buffer its accumulators completely (3 slots of
-    // 160 TMEM columns): the drain of its first sub-tile is exposed
-    const long cost = waves * (kb * kiters + (ns == 2 ? 4000 : 1000));
-    if (best == 0 || cost < best_cost) best = w, best_cost = cost;
+// Tile width BN (the wgmma N).  The K order of every output element is the same for every width, so the width is a pure
+// scheduling choice and depends on N only: 128 where it divides N (two 64 x 128 fp32 accumulator blocks per CTA leave
+// room for a deep operand ring), otherwise the widest divisor of N among 160 / 192 / 96 / 64 / 32 (N = 320, 960, ...).
+// GEGLU tiles hold [BN/2 linear | BN/2 gate] and must match the weight permutation (ddpo_prep_weight geglu_bn).
+static int pick_width(int N, int geglu) {
+  if (geglu) {
+    for (int w : {256, 192, 128, 64})
+      if (N % w == 0) return w;
+    return 0;
   }
-  return best;
+  for (int w : {128, 160, 192, 96, 64, 32})
+    if (N % w == 0) return w;
+  return 0;
+}
+
+template <int BN>
+static int igemm_launch(IGemmArgs& p, cudaStream_t stream) {
+  constexpr int SB = igemm_stage_bytes<BN>();
+  constexpr int EPI = igemm_epi_bytes<BN>();
+  // Three or more stages in half the shared memory: two CTAs per SM, so that one CTA's epilogue overlaps the other's
+  // main loop.  Otherwise one CTA with as many stages as fit.
+  int stages = (110 * 1024) / SB;
+  if (BN > 128 || stages < 3 || stages * SB < EPI) stages = SMEM_BUDGET / SB;
+  if (stages > 8) stages = 8;
+  DDPO_REQUIRE(stages >= 2, "ddpo_igemm: not enough shared memory for BN=%d", BN);
+  p.stages = stages;
+  const size_t smem = (size_t)(stages * SB > EPI ? stages * SB : EPI) + 256 + 1024;
+  static bool attr_set = false;
+  if (!attr_set) {
+    DDPO_CUDA_OK(cudaFuncSetAttribute(igemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    attr_set = true;
+  }
+  const int tiles = ((p.M_total + BM - 1) / BM) * (p.N_total / BN);
+  igemm_kernel<BN><<<tiles, IGEMM_THREADS, smem, stream>>>(p);
+  DDPO_LAUNCH_OK();
+  return DDPO_OK;
 }
 
 }  // namespace ddpo
 
 using namespace ddpo;
-
-int ddpo_igemm2_launch(IGemmArgs& p, cudaStream_t stream);  // igemm2.cu
 
 extern "C" int ddpo_igemm(const ddpo_igemm_args* a, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
@@ -254,26 +285,11 @@ extern "C" int ddpo_igemm(const ddpo_igemm_args* a, void* stream_) {
   DDPO_REQUIRE(a->taps == 1 || a->taps == 9, "ddpo_igemm: taps must be 1 or 9");
   DDPO_REQUIRE(a->n % 32 == 0, "ddpo_igemm: N=%d must be a multiple of 32", a->n);
   DDPO_REQUIRE(a->out_f32 != nullptr || a->out_bf16 != nullptr, "ddpo_igemm: no output");
-  const int m_rows = a->is_conv ? a->batch * a->w * a->h : a->m;
-  // CTA pairs (cta_group::2, 256 x BN tiles) whenever the problem has enough rows; see igemm2.cu
-  const bool use_pair = a->pair_override == 1 || (a->pair_override == 0 && a->mt_override == 0 && m_rows >= 1024);
-  // DDPO_IGEMM_WIDE=0 keeps every tile at one UMMA width (A/B switch for the 2 x 160 tiles)
-  static const bool allow_wide = []() {
-    const char* e = getenv("DDPO_IGEMM_WIDE");
-    return e == nullptr || e[0] != '0';
-  }();
-  int BN = a->bn_override > 0 ? a->bn_override
-                              : pick_width(a->n, a->geglu, m_rows, a->taps * (cin0 + cin1) / BK, use_pair,
-                                           // short-K layers run the TMA-staged epilogue, whose buffers leave too few stages
-                                           allow_wide && a->epi_override != 1 &&
-                                               (a->epi_override == 2 || a->taps * (cin0 + cin1) / BK > 24));
-  int NS = 1;
-  if (BN > 256) {  // bn_override = 320 (or the cost model): two sub-tiles of 160 columns per CTA-pair tile
-    DDPO_REQUIRE(BN == 320 && use_pair && !a->geglu, "ddpo_igemm: 320-wide tiles need the CTA-pair kernel and no GEGLU");
-    DDPO_REQUIRE(a->n % 320 == 0, "ddpo_igemm: N=%d is not a multiple of 320", a->n);
-    NS = 2, BN = 160;
-  }
-  DDPO_REQUIRE(BN > 0 && a->n % BN == 0 && BN % 32 == 0 && BN <= 256, "ddpo_igemm: no valid BN for N=%d", a->n);
+  int BN = a->bn_override > 0 ? a->bn_override : pick_width(a->n, a->geglu);
+  if (BN == 320 && !a->geglu) BN = 160;  // a 320-wide tile is two 160-column tiles
+  DDPO_REQUIRE(BN == 32 || BN == 64 || BN == 96 || BN == 128 || BN == 160 || BN == 192 || BN == 256,
+               "ddpo_igemm: unsupported tile width %d", BN);
+  DDPO_REQUIRE(a->n % BN == 0, "ddpo_igemm: no valid BN for N=%d", a->n);
   if (a->geglu) DDPO_REQUIRE(BN % 64 == 0 && a->out_bf16 != nullptr && a->bias != nullptr, "ddpo_igemm: bad GEGLU config");
 
   IGemmArgs p;
@@ -286,9 +302,8 @@ extern "C" int ddpo_igemm(const ddpo_igemm_args* a, void* stream_) {
     DDPO_REQUIRE(s == 1 || s == 2, "ddpo_igemm: stride must be 1 or 2");
     DDPO_REQUIRE(W > 0 && H > 0 && (W & (W - 1)) == 0 && (H & (H - 1)) == 0 && W <= 1024,
                  "ddpo_igemm: W,H must be powers of two, W<=1024 (W=%d H=%d)", W, H);
-    // rows wider than a tile are cut into W/128 tiles; with stride 2 the 128-pixel box spans 256 input elements (the TMA limit)
-    DDPO_REQUIRE(W <= BM || a->mt_override == 0, "ddpo_igemm: rows wider than %d pixels cannot use 256-row CTA tiles (W=%d)", BM, W);
-    // a 128-row tile is bb samples x bh rows x bw pixels; rows wider than the tile are cut into W/128 tiles
+    // a 128-row tile is bb samples x bh rows x bw pixels; rows wider than the tile are cut into W/128 tiles (with
+    // stride 2 the 128-pixel box spans 256 input elements, the TMA limit)
     int bw = W < BM ? W : BM, bh = (BM / bw < H) ? BM / bw : H;
     int bb = BM / (bw * bh);
     M_total = B * W * H;
@@ -322,12 +337,12 @@ extern "C" int ddpo_igemm(const ddpo_igemm_args* a, void* stream_) {
   {
     uint64_t dims[2] = {(uint64_t)ktot, (uint64_t)a->n};
     uint64_t strides[1] = {(uint64_t)ktot * 2};
-    uint32_t box[2] = {(uint32_t)BK, (uint32_t)(use_pair ? BN / 2 : BN)};
+    uint32_t box[2] = {(uint32_t)BK, (uint32_t)BN};
     uint32_t es[2] = {1, 1};
     int rc = make_tensor_map(&p.tmB, a->wt, 2, 2, dims, strides, box, es, 1);
     if (rc) return rc;
   }
-  p.M_total = M_total, p.N_total = a->n, p.BN = BN, p.NS = NS;
+  p.M_total = M_total, p.N_total = a->n;
   p.taps = a->taps, p.kc0 = cin0 / BK, p.kc1 = cin1 / BK, p.is_conv = a->is_conv;
   p.bias = a->bias, p.rowvec = a->rowvec, p.rows_per_sample = a->rows_per_sample > 0 ? a->rows_per_sample : 1;
   p.rowvec_ld = a->rowvec_ld;
@@ -337,88 +352,23 @@ extern "C" int ddpo_igemm(const ddpo_igemm_args* a, void* stream_) {
   p.geglu = a->geglu, p.accumulate_out = a->accumulate_out;
   p.aux_bf16 = static_cast<__nv_bfloat16*>(a->aux_bf16);
   p.gn_stats = a->gn_stats;
+  // the epilogue moves four columns per access: 16-byte fp32 / 8-byte bf16 vectors
+  const auto aligned = [](const void* ptr, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(ptr) & (bytes - 1)) == 0; };
+  DDPO_REQUIRE(aligned(a->out_f32, 16) && aligned(a->residual, 16) && aligned(a->bias, 16) && aligned(a->rowvec, 16) &&
+                   aligned(a->gn_stats, 8) && aligned(a->out_bf16, 8) && aligned(a->aux_bf16, 8),
+               "ddpo_igemm: out_f32 / residual / bias / rowvec must be 16-byte aligned, out_bf16 / aux_bf16 / gn_stats 8-byte aligned");
+  DDPO_REQUIRE(p.ld_out % 4 == 0 && p.ld_res % 4 == 0 && (a->rowvec == nullptr || a->rowvec_ld % 4 == 0),
+               "ddpo_igemm: ld_out (%d), ld_res (%d) and rowvec_ld (%d) must be multiples of 4", p.ld_out, p.ld_res, a->rowvec_ld);
   if (a->gn_stats != nullptr)
     DDPO_REQUIRE(a->out_f32 != nullptr && !a->geglu && !a->accumulate_out,
                  "ddpo_igemm: gn_stats describes a plain fp32 output (no GEGLU, no accumulate)");
-  {
-    // DDPO_IGEMM_STAGED=0: register epilogue with one row per lane (A/B switch)
-    static const bool staged = []() {
-      const char* e = getenv("DDPO_IGEMM_STAGED");
-      return e == nullptr || e[0] != '0';
-    }();
-    p.epi_stage = staged && !a->geglu && p.ld_out % 8 == 0 && p.ld_res % 4 == 0 &&
-                  (reinterpret_cast<uintptr_t>(a->out_f32) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->out_bf16) & 15) == 0 &&
-                  (reinterpret_cast<uintptr_t>(a->residual) & 15) == 0;
+  switch (BN) {
+    case 32: return igemm_launch<32>(p, stream);
+    case 64: return igemm_launch<64>(p, stream);
+    case 96: return igemm_launch<96>(p, stream);
+    case 128: return igemm_launch<128>(p, stream);
+    case 160: return igemm_launch<160>(p, stream);
+    case 192: return igemm_launch<192>(p, stream);
+    default: return igemm_launch<256>(p, stream);
   }
-  if (use_pair) {
-    p.MT = 1;
-    {
-      const char* e = getenv("DDPO_IGEMM_DEBUG");
-      p.dbg = e != nullptr ? atoi(e) : 0;
-      e = getenv("DDPO_IGEMM_PREFETCH");
-      p.res_prefetch = e == nullptr || e[0] != '0';
-    }
-    // TMA epilogue where the epilogue, not the main loop, bounds the tile: short K (the 1x1 / linear layers).
-    // Long-K convolutions hide the register epilogue behind the next tile's MMAs and keep every stage for operands.
-    const int kiters = a->taps * (cin0 + cin1) / BK;
-    const bool aligned = (reinterpret_cast<uintptr_t>(a->out_f32) & 15) == 0 &&
-                         (reinterpret_cast<uintptr_t>(a->out_bf16) & 15) == 0 &&
-                         (reinterpret_cast<uintptr_t>(a->residual) & 15) == 0 &&
-                         (reinterpret_cast<uintptr_t>(a->aux_bf16) & 15) == 0 && p.ld_out % 8 == 0 && p.ld_res % 4 == 0;
-    const bool can_tma = aligned && !(a->residual != nullptr && a->accumulate_out) &&
-                         (!a->geglu || (a->residual == nullptr && !a->accumulate_out && a->out_f32 == nullptr));
-    const bool want_tma = a->epi_override == 1 || (a->epi_override == 0 && kiters <= 24);
-    if (can_tma && want_tma) {
-      p.epi_tma = 1, p.epi_stage = 0;
-      uint32_t box[2] = {32, 32}, es[2] = {1, 1};
-      int rc;
-      if (a->geglu) {
-        uint64_t dims_o[2] = {(uint64_t)a->n / 2, (uint64_t)M_total}, st_o[1] = {(uint64_t)p.ld_out * 2};
-        if ((rc = make_tensor_map(&p.tmOutB, a->out_bf16, 2, 2, dims_o, st_o, box, es, 2))) return rc;
-        if (a->aux_bf16 != nullptr) {
-          uint64_t dims_a[2] = {(uint64_t)a->n, (uint64_t)M_total}, st_a[1] = {(uint64_t)a->n * 2};
-          if ((rc = make_tensor_map(&p.tmIn, a->aux_bf16, 2, 2, dims_a, st_a, box, es, 2))) return rc;
-        }
-      } else {
-        const float* in = a->residual != nullptr ? a->residual : (a->accumulate_out ? a->out_f32 : nullptr);
-        const int ld_in = a->residual != nullptr ? p.ld_res : p.ld_out;
-        p.epi_in = in != nullptr;
-        uint64_t dims[2] = {(uint64_t)a->n, (uint64_t)M_total};
-        if (in != nullptr) {
-          uint64_t st[1] = {(uint64_t)ld_in * 4};
-          if ((rc = make_tensor_map(&p.tmIn, in, 4, 2, dims, st, box, es, 1))) return rc;
-        }
-        if (a->out_f32 != nullptr) {
-          uint64_t st[1] = {(uint64_t)p.ld_out * 4};
-          if ((rc = make_tensor_map(&p.tmOutF, a->out_f32, 4, 2, dims, st, box, es, 1))) return rc;
-        }
-        if (a->out_bf16 != nullptr) {
-          uint64_t st[1] = {(uint64_t)p.ld_out * 2};
-          if ((rc = make_tensor_map(&p.tmOutB, a->out_bf16, 2, 2, dims, st, box, es, 2))) return rc;
-        }
-      }
-    }
-    return ddpo_igemm2_launch(p, stream);
-  }
-  // fat tiles (BM = 256) when there are still >= 2 waves of them and the main loop is long enough to amortise the
-  // non-overlapped epilogue: operand bytes per MMA cycle drop from 8192(1/128+1/BN) to 8192(1/256+1/BN)
-  int MT = (a->mt_override > 0) ? a->mt_override : 1;
-  p.MT = MT;
-  const int stage_bytes = MT * A_TILE_BYTES + BN * BK * 2;
-  int stages = (SMEM_BUDGET - (p.epi_stage ? EPI_STAGE_BYTES : 0)) / stage_bytes;
-  if (stages > 8) stages = 8;
-  DDPO_REQUIRE(stages >= 2, "ddpo_igemm: not enough shared memory for BN=%d MT=%d", BN, MT);
-  p.stages = stages;
-  const size_t smem = (size_t)stages * stage_bytes + 256 + 1024 + (p.epi_stage ? EPI_STAGE_BYTES : 0);
-  static bool attr_set = false;
-  if (!attr_set) {
-    DDPO_CUDA_OK(cudaFuncSetAttribute(igemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-  const int tiles = ((M_total + BM * MT - 1) / (BM * MT)) * (a->n / BN);
-  int grid = num_sms();
-  if (grid > tiles) grid = tiles;
-  igemm_kernel<<<grid, IGEMM_THREADS, smem, stream>>>(p);
-  DDPO_LAUNCH_OK();
-  return DDPO_OK;
 }

@@ -10,7 +10,7 @@
 // U-Net skip connection is never materialised), y bf16 (the next GEMM's A operand).
 //
 // Statistics.  The GEMM that PRODUCES x leaves per-(32-row slab, channel) sums and sums of squares of what it writes
-// (igemm_common.cuh gn_slab_stats); gn_finalize_slabs_kernel folds them, in a fixed order, into one (mean, rstd) pair per
+// (igemm.cu epilogue); gn_finalize_slabs_kernel folds them, in a fixed order, into one (mean, rstd) pair per
 // (sample, group) -- so the forward pass reads x ONCE (algorithmic traffic: 4 B in + 2 B out per element) instead of
 // once for the statistics and once more for the normalisation.  Inputs without slab statistics (conv_in's output, the VAE
 // decoder, grids with fewer than 32 pixels) go through gn_stats_kernel (per (sample, pixel-chunk) partial sums) and
@@ -125,8 +125,8 @@ __global__ void __launch_bounds__(GNF_THREADS) gn_finalize_slabs_kernel(const Gn
   const int nslab = a.hw >> 5;
   const int items = nslab * cpg;
   float s = 0.f, ss = 0.f;
-  // eight independent loads per thread in flight (a plain accumulate loop serialises on the load latency: 10 us for the
-  // 5 MB of statistics of a 64x64x320 batch of 16), summed in ascending item order
+  // eight independent loads per thread in flight (a plain accumulate loop serialises on the load
+  // latency), summed in ascending item order
   for (int base = threadIdx.x; base < items; base += GNF_THREADS * 8) {
     float2 v[8];
 #pragma unroll
@@ -177,7 +177,7 @@ __global__ void gn_finalize_chunks_kernel(const GnArgs a, int batch) {
 // Per-element arithmetic shared by the two apply kernels (bit-identical outputs whichever runs): the affine part as ONE
 // fused multiply-add y = x * A + B with A = rstd * scale, B = bias - mean * A (per thread and channel, computed once), SiLU
 // on one MUFU op when the only consumer is the bf16 GEMM operand.  The apply pass was issue- / MUFU-bound with the
-// three-instruction affine and the two-MUFU sigmoid (measured: 58 us for 126 MB, profiles/r2_norm.md).
+// three-instruction affine and the two-MUFU sigmoid.
 __device__ __forceinline__ void gn_coef(float mean, float rstd, float scale, float bias, float& A, float& B) {
   A = rstd * scale;
   B = fmaf(-mean, A, bias);
@@ -357,8 +357,7 @@ struct GnBwdArgs {
 };
 
 // four consecutive gradient values at element index `idx` (a multiple of 4).  The element type is a TEMPLATE parameter of
-// the kernels: with a run-time branch inside the unrolled load loops the compiler stopped batching the row's loads (the
-// LayerNorm backward went from 11.5 to 19.3 ms per train pass).
+// the kernels: with a run-time branch inside the unrolled load loops the compiler stops batching the row's loads.
 template <bool BF16>
 __device__ __forceinline__ float4 gn_load_dy4(const void* dy, size_t idx) {
   if (BF16) {
@@ -680,7 +679,7 @@ __global__ void __launch_bounds__(256) layernorm_bwd_kernel(const float* __restr
 
 static int gn_chunking(int hw, int* chunks, int* ppc) {
   // 32 chunks per sample for the U-Net's grids (hw <= 4096); at most 512 pixels per chunk beyond that, so the VAE
-  // decoder's 128^2 .. 512^2 levels (2-image chunks) still launch enough CTAs to fill 148 SMs.  The chunking depends
+  // decoder's 128^2 .. 512^2 levels (2-image chunks) still launch enough CTAs to fill 132 SMs.  The chunking depends
   // on hw only -> reduction order (and the result bits) are independent of the batch size.
   int p = hw / 32;
   if (p > 512) p = 512;
@@ -730,10 +729,8 @@ extern "C" int64_t ddpo_groupnorm_workspace_floats(int batch, int hw, int channe
 
 // plan of the streamed apply pass; returns false when the shape does not fit it (the two-pass kernels then run)
 static bool gn_stream_plan(const GnArgs& g, const ddpo_groupnorm_args* a, GnStream* st) {
-  // Opt-in ($DDPO_GN_STREAM=1; read per call: the bit-identity test toggles it).  Measured on B200 after the apply
-  // arithmetic was cut to one FMA + one MUFU per element (profiles/r2_norm.md): the plain kernel (960 threads / SM issuing
-  // their own 16-byte loads) moves 126 MB in 29.2 us and 315 MB in 62.1 us (5.07 TB/s = 0.77 of the copy peak); this
-  // TMA-staged one, with 20 consumer warps per SM, 34.8 / 72.2 us -- the pass is issue-bound before it is latency-bound.
+  // Opt-in ($DDPO_GN_STREAM=1; read per call: the bit-identity test toggles it).  The plain kernel (every thread issuing
+  // its own 16-byte loads) is the default; this TMA-staged one is kept as a developer A/B switch.
   const char* on = getenv("DDPO_GN_STREAM");
   if (on == nullptr || on[0] != '1') return false;
   const int nsrc = a->c1 > 0 ? 2 : 1;

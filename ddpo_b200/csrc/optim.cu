@@ -12,7 +12,7 @@
 
 namespace ddpo {
 
-constexpr int NORM_BLOCKS = 1184;  // 148 SMs x 8
+constexpr int NORM_BLOCKS = 1056;  // 132 SMs (H100 SXM) x 8
 
 __global__ void __launch_bounds__(256) sumsq_partial_kernel(const float* __restrict__ g, int64_t n4, double* __restrict__ part) {
   float acc = 0.f;
@@ -107,7 +107,7 @@ extern "C" int ddpo_clip_adamw(float* params, float* grad_acc, void* mu_bf16, fl
   a.bc1 = static_cast<float>(1.0 - pow(static_cast<double>(b1), step));
   a.bc2 = static_cast<float>(1.0 - pow(static_cast<double>(b2), step));
   a.norm_out = norm_out;
-  clip_adamw_kernel<<<148 * 8, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
+  clip_adamw_kernel<<<NORM_BLOCKS, 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
   DDPO_LAUNCH_OK();
   return DDPO_OK;
 }

@@ -4,8 +4,7 @@
 // Deterministic: thread (tx, ty) of a 32 x 32 block adds rows ty, ty + 32, ... of column tx in ascending order and the
 // 32 per-thread sums are combined in ascending ty through shared memory -- the result depends only on (rows, width),
 // never on timing.  The first-stage kernels emit up to 2560 partial rows for the 64 x 64 feature maps; the previous
-// one-thread-per-column loop over them (3 CTAs of 128 threads) took 50-150 us per launch, 24 ms per train pass
-// (profiles/r1_launches_summary.md); here every warp reads 128 contiguous bytes per row and 32 rows are in flight
+// one-thread-per-column loop over them (3 CTAs of 128 threads) was latency-bound; here every warp reads 128 contiguous bytes per row and 32 rows are in flight
 // per column.
 #pragma once
 #include "common.cuh"

@@ -85,7 +85,7 @@ extern "C" int ddpo_embed_tokens(const int32_t* ids, const float* token_embeddin
 extern "C" int ddpo_act_bf16(const float* x, void* y_bf16, int64_t n, int act, void* stream) {
   DDPO_REQUIRE(x && y_bf16 && n > 0 && n % 4 == 0 && (act == 0 || act == 1), "act_bf16: bad arguments");
   int64_t blocks = (n / 4 + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   act_bf16_kernel<<<static_cast<int>(blocks), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       x, static_cast<__nv_bfloat16*>(y_bf16), n / 4, act);
   DDPO_LAUNCH_OK();

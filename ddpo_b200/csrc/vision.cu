@@ -62,7 +62,7 @@ using namespace ddpo;
 
 static inline int vgrid(int64_t n) {
   int64_t g = (n + 255) / 256;
-  return static_cast<int>(g > 148 * 32 ? 148 * 32 : (g < 1 ? 1 : g));
+  return static_cast<int>(g > 132 * 32 ? 132 * 32 : (g < 1 ? 1 : g));
 }
 
 extern "C" int ddpo_patchify_bf16(const float* img_nhwc, void* out_bf16, int batch, int size, int patch, int ldk,

@@ -1,4 +1,4 @@
-// Weight-gradient GEMM on tcgen05:  dW[(tap, c_in), c_out] += sum_pixels X[pixel + tap, c_in] * dY[pixel, c_out]
+// Weight-gradient GEMM on wgmma (sm_90a):  dW[(tap, c_in), c_out] += sum_pixels X[pixel + tap, c_in] * dY[pixel, c_out]
 //
 // Backward of nn.Conv / nn.Dense of the 3P Flax U-Net w.r.t. their kernels -- the part of
 // `jax.grad(compute_loss)` (reference ddpo/training/policy_gradient.py:138) that XLA emits as
@@ -6,18 +6,20 @@
 // parameter layout (HWIO == [(tap, c_in), c_out]; Dense [in, out]) and ACCUMULATED into the flat
 // fp32 gradient buffer, so `grad_acc += g` (AccumulatingTrainState, :44-47) costs no extra pass.
 //
-// The reduction (UMMA K) dimension is the pixel index, which is the slow dimension of both NHWC
+// The reduction (wgmma K) dimension is the pixel index, which is the slow dimension of both NHWC
 // operands -> both operands are "MN-major": TMA boxes of [64 pixels x 64 channels] land as
-// 128-byte rows (SWIZZLE_128B) and are consumed through MN-major UMMA descriptors
-// (LBO = 8 KB between 64-channel groups, SBO = 1 KB between 8-pixel groups).  As in the forward
+// 128-byte rows (SWIZZLE_128B) and are consumed through transposed wgmma descriptors
+// (LBO = 8 KB between 64-channel boxes, SBO = 1 KB between 8-pixel groups).  As in the forward
 // kernel the 3x3 taps are shifted boxes with TMA zero fill as padding.
+// One CTA = 128 input channels (two consumer warpgroups of 64) x BN output channels; warp 8 is the TMA producer.
 // Pixels are split into `splits` fixed ranges to fill the machine; partial tiles go to a workspace
 // and are summed in split order by a second kernel (deterministic, no atomics).
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace ddpo {
 
-constexpr int WG_THREADS = 384;  // warps 4-11: epilogue (alternating 32-column chunks)
+constexpr int WG_THREADS = 288;                    // warps 0-7: two consumer warpgroups, warp 8: TMA producer
 constexpr int WG_BKP = 64;                         // pixels per pipeline stage
 constexpr int WG_BOX_BYTES = WG_BKP * 64 * 2;      // [64 pixels x 64 channels] bf16 = 8 KB
 constexpr int WG_A_BYTES = 2 * WG_BOX_BYTES;       // 128 input channels
@@ -27,197 +29,127 @@ struct WgradKArgs {
   CUtensorMap tmX0, tmX1, tmDY;
   int c0, c1, n;              // input channels per source, output channels
   int taps, is_conv, W, H, conv_stride, pad;
-  int pix_total;              // rows of dY
   int splits, pblocks_per_split, pblocks;
   int mt_per_tap0, mt_per_tap1;  // 128-channel blocks per source
+  int n_begin, NT;            // this launch: NT column tiles of BN from column n_begin
   int stages;
   float* dst;                 // splits == 1: dW (+=) ; else workspace [splits][rows][n]
   int accumulate;
 };
 
-__device__ __forceinline__ int wg_bn(int n, int nt) {  // N tiles of 256 + remainder (multiple of 64)
-  const int rem = n - nt * 256;
-  return rem >= 256 ? 256 : rem;
-}
-
+template <int BN>
 __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_kernel(const __grid_constant__ WgradKArgs p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  constexpr int SB = WG_A_BYTES + BN * 128;
   const int stages = p.stages;
-  const int stage_bytes = WG_A_BYTES + 4 * WG_BOX_BYTES;  // A (16 KB) + up to 256 dY channels (32 KB)
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + stages * stage_bytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + stages * SB);
   uint64_t* empty_bar = full_bar + stages;
-  uint64_t* tmem_full = empty_bar + stages;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty + 2);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
+  // tile -> (split, tap, source, channel block, n tile)
   const int mt_per_tap = p.mt_per_tap0 + p.mt_per_tap1;
   const int MT = p.taps * mt_per_tap;
-  const int NT = (p.n + 255) / 256;
-  const int num_tiles = p.splits * MT * NT;
-  const int cin = p.c0 + p.c1;
+  const int tile = blockIdx.x;
+  const int nt = tile % p.NT;
+  const int mt = (tile / p.NT) % MT;
+  const int s = tile / p.NT / MT;
+  const int tap = mt / mt_per_tap;
+  const int mb = mt % mt_per_tap;
+  const int src = mb >= p.mt_per_tap0;
+  const int blk = src ? mb - p.mt_per_tap0 : mb;
+  const int ncol0 = p.n_begin + nt * BN;
+  const int pb0 = s * p.pblocks_per_split;
+  const int pb1 = min(p.pblocks, pb0 + p.pblocks_per_split);
 
-  if (warp == 0 && lane == 0) {
-    prefetch_tmap(&p.tmX0);
-    prefetch_tmap(&p.tmX1);
-    prefetch_tmap(&p.tmDY);
-  }
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
     for (int i = 0; i < stages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 8);
+      mbar_init(&empty_bar[i], 8);
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  // tile -> (split, tap, source, channel block, n tile)
-  auto decode = [&](int tile, int& s, int& tap, int& src, int& blk, int& nt) {
-    nt = tile % NT;
-    int r = tile / NT;
-    const int mt = r % MT;
-    s = r / MT;
-    tap = mt / mt_per_tap;
-    const int mb = mt % mt_per_tap;
-    src = mb >= p.mt_per_tap0;
-    blk = src ? mb - p.mt_per_tap0 : mb;
-  };
-
-  // single-role warps run their loops converged and elect a lane for the issue instructions only (operands stay in
-  // uniform registers; see igemm2.cu)
-  if (warp == 0) {
-    {
-      int stage = 0;
-      uint32_t phase = 0;
+  if (warp == 8) {
+    if (lane == 0) {
+      prefetch_tmap(&p.tmX0);
+      prefetch_tmap(&p.tmX1);
+      prefetch_tmap(&p.tmDY);
       const int HW = p.W * p.H;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int s, tap, src, blk, nt;
-        decode(tile, s, tap, src, blk, nt);
-        const int bn = wg_bn(p.n, nt);
-        const int pb0 = s * p.pblocks_per_split;
-        const int pb1 = min(p.pblocks, pb0 + p.pblocks_per_split);
-        int dy = 0, dx = 0;
-        if (p.taps == 9) dy = tap / 3, dx = tap - dy * 3;
-        const CUtensorMap* tmX = src ? &p.tmX1 : &p.tmX0;
-        for (int pb = pb0; pb < pb1; ++pb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sA = smem + stage * stage_bytes;
-          uint8_t* sB = sA + WG_A_BYTES;
-          const int row0 = pb * WG_BKP;
-          if (elect_one()) {
-            mbar_expect_tx(&full_bar[stage], WG_A_BYTES + (bn / 64) * WG_BOX_BYTES);
-            if (p.is_conv) {
-              const int b0 = row0 / HW, h0 = (row0 % HW) / p.W;
-              const int cx = dx - p.pad, cy = h0 * p.conv_stride + dy - p.pad;
-              tma_load_4d(sA, tmX, &full_bar[stage], blk * 128, cx, cy, b0);
-              tma_load_4d(sA + WG_BOX_BYTES, tmX, &full_bar[stage], blk * 128 + 64, cx, cy, b0);
-            } else {
-              tma_load_2d(sA, tmX, &full_bar[stage], blk * 128, row0);
-              tma_load_2d(sA + WG_BOX_BYTES, tmX, &full_bar[stage], blk * 128 + 64, row0);
-            }
-            for (int j = 0; j < bn / 64; ++j)
-              tma_load_2d(sB + j * WG_BOX_BYTES, &p.tmDY, &full_bar[stage], nt * 256 + j * 64, row0);
-          }
-          __syncwarp();
-          if (++stage == stages) stage = 0, phase ^= 1;
-        }
-      }
-    }
-  } else if (warp == 1) {
-    {
+      int dy = 0, dx = 0;
+      if (p.taps == 9) dy = tap / 3, dx = tap - dy * 3;
+      const CUtensorMap* tmX = src ? &p.tmX1 : &p.tmX0;
       int stage = 0;
       uint32_t phase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        int s, tap, src, blk, nt;
-        decode(tile, s, tap, src, blk, nt);
-        const int bn = wg_bn(p.n, nt);
-        const uint32_t idesc = umma_idesc_bf16(128, bn, 1, 1);  // both operands MN-major
-        const int pb0 = s * p.pblocks_per_split;
-        const int pb1 = min(p.pblocks, pb0 + p.pblocks_per_split);
-        const int buf = it & 1;
-        mbar_wait(&tmem_empty[buf], ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * 256;
-        for (int pb = pb0; pb < pb1; ++pb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_base = smem_u32(smem + stage * stage_bytes);
-          const uint32_t b_base = a_base + WG_A_BYTES;
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < WG_BKP / 16; ++k) {
-              // 16 pixels = 16 rows of 128 B; LBO = stride between 64-channel groups, SBO = 8-row groups
-              umma_bf16(d_tmem, umma_desc(a_base + k * 2048, WG_BOX_BYTES, 1024),
-                        umma_desc(b_base + k * 2048, WG_BOX_BYTES, 1024), idesc, (pb > pb0 || k > 0) ? 1u : 0u);
-            }
-            umma_commit(&empty_bar[stage]);
-          }
-          __syncwarp();
-          if (++stage == stages) stage = 0, phase ^= 1;
+      for (int pb = pb0; pb < pb1; ++pb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        uint8_t* sA = smem + stage * SB;
+        uint8_t* sB = sA + WG_A_BYTES;
+        const int row0 = pb * WG_BKP;
+        mbar_expect_tx(&full_bar[stage], SB);
+        if (p.is_conv) {
+          const int b0 = row0 / HW, h0 = (row0 % HW) / p.W;
+          const int cx = dx - p.pad, cy = h0 * p.conv_stride + dy - p.pad;
+          tma_load_4d(sA, tmX, &full_bar[stage], blk * 128, cx, cy, b0);
+          tma_load_4d(sA + WG_BOX_BYTES, tmX, &full_bar[stage], blk * 128 + 64, cx, cy, b0);
+        } else {
+          tma_load_2d(sA, tmX, &full_bar[stage], blk * 128, row0);
+          tma_load_2d(sA + WG_BOX_BYTES, tmX, &full_bar[stage], blk * 128 + 64, row0);
         }
-        if (elect_one()) umma_commit(&tmem_full[buf]);
-        __syncwarp();
+        for (int j = 0; j < BN / 64; ++j) tma_load_2d(sB + j * WG_BOX_BYTES, &p.tmDY, &full_bar[stage], ncol0 + j * 64, row0);
+        if (++stage == stages) stage = 0, phase ^= 1;
       }
     }
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    const int cgrp = (warp - 4) >> 2;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      int s, tap, src, blk, nt;
-      decode(tile, s, tap, src, blk, nt);
-      const int bn = wg_bn(p.n, nt);
-      const int buf = it & 1;
-      mbar_wait(&tmem_full[buf], (it >> 1) & 1);
-      tc_fence_after();
-      const int ch = blk * 128 + q * 32 + lane;          // input channel within the source
-      const int csrc = src ? p.c1 : p.c0;
-      const bool ok = ch < csrc;
-      const size_t row = static_cast<size_t>(tap) * cin + (src ? p.c0 : 0) + ch;
-      const size_t rows_total = static_cast<size_t>(p.taps) * cin;
-      float* dst = p.dst + (p.splits > 1 ? static_cast<size_t>(s) * rows_total * p.n : 0) + row * p.n + nt * 256;
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + buf * 256;
-      for (int c0 = cgrp * 32; c0 < bn; c0 += 64) {
-        uint32_t v[32];
-        tmem_ld_32x32(t_row + c0, v);
-        tmem_ld_wait();
-        if (ok) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            float4 o = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
-                                   __uint_as_float(v[j + 3]));
-            float4* d = reinterpret_cast<float4*>(dst + c0 + j);
-            if (p.splits == 1 && p.accumulate) {
-              const float4 old = *d;
-              o.x += old.x, o.y += old.y, o.z += old.z, o.w += old.w;
-            }
-            *d = o;
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[buf]);
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+
+  const int wg = warp >> 2;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  {
+    int stage = 0, prev = 0;
+    uint32_t phase = 0;
+    for (int pb = pb0; pb < pb1; ++pb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t a_base = smem_u32(smem + stage * SB) + wg * WG_BOX_BYTES;
+      const uint32_t b_base = smem_u32(smem + stage * SB) + WG_A_BYTES;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < WG_BKP / 16; ++k)  // 16 pixels = 16 rows of 128 B
+        Wgmma<BN>::template ss<1, 1>(acc, gmma_desc(a_base + k * 2048, WG_BOX_BYTES, 1024),
+                                     gmma_desc(b_base + k * 2048, WG_BOX_BYTES, 1024), (pb > pb0 || k > 0) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (pb > pb0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == stages) stage = 0, phase ^= 1;
+    }
+    wgmma_wait<0>();
+  }
+
+  // accumulator fragment: rows (input channels) r0 and r0 + 8, columns 8 j + 2 (lane & 3) + {0, 1}
+  const int cin = p.c0 + p.c1;
+  const int csrc = src ? p.c1 : p.c0;
+  const size_t rows_total = static_cast<size_t>(p.taps) * cin;
+  float* base = p.dst + (p.splits > 1 ? static_cast<size_t>(s) * rows_total * p.n : 0) + ncol0 + 2 * (lane & 3);
+  const bool acc_old = p.splits == 1 && p.accumulate;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int ch = blk * 128 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;  // input channel within the source
+    if (ch >= csrc) continue;
+    float* d = base + (static_cast<size_t>(tap) * cin + (src ? p.c0 : 0) + ch) * p.n;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      float2 o = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+      float2* dp = reinterpret_cast<float2*>(d + 8 * j);
+      if (acc_old) {
+        const float2 old = *dp;
+        o.x += old.x, o.y += old.y;
+      }
+      *dp = o;
+    }
   }
 }
 
@@ -238,54 +170,40 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ part, float* __res
 
 using namespace ddpo;
 
-int ddpo_wgrad2_tiles(int taps, int cin, int n);  // wgrad2.cu
-int ddpo_wgrad2_launch(const CUtensorMap& tmX0, const CUtensorMap& tmX1, const CUtensorMap& tmDY, int c0, int c1, int n,
-                       int taps, int is_conv, int W, int H, int conv_stride, int splits, int pblocks, float* dst,
-                       cudaStream_t stream);
-
-static bool wgrad_use_pair(const ddpo_wgrad_args* a) { return a->kernel_override != 2; }
-
 static int wgrad_plan(const ddpo_wgrad_args* a, int* splits, int* pblocks) {
   const int m = a->is_conv ? a->batch * a->h * a->w : a->m;
   const int pb = (m + WG_BKP - 1) / WG_BKP;
   const int cin = a->c0 + a->c1;
-  int s;
-  if (wgrad_use_pair(a)) {
-    // CTA-pair kernel, 74 pairs.  Number of pixel splits from a small cost model (microseconds):
-    //   main loop  = rounds x pixel blocks per split x 0.42 us per 256-wide 64-pixel stage (measured; 0.6 of that for
-    //                the 128-wide padded remainder tile)
-    //   reduction  = (splits + 2) x |dW| x 4 B at ~4 TB/s (partials written, read back, dW read-modify-written)
-    const int tiles = ddpo_wgrad2_tiles(a->taps, cin, a->n);
-    const int workers = num_sms() / 2;
-    const int nt = (a->n + 255) / 256;
-    const double wide = (a->n - (nt - 1) * 256) > 128 ? 1.0 : 0.6;
-    const double stage_us = 0.42 * ((nt - 1) + wide) / nt;
-    const double dw_mb = static_cast<double>(a->taps) * cin * a->n * 4.0 / 1e6;
-    int hi = pb / 4;
-    if (hi < 1) hi = 1;
-    if (hi > 64) hi = 64;
-    s = 1;
-    double best = 1e30;
-    for (int sk = 1; sk <= hi; ++sk) {
-      const int units = sk * tiles;
-      const int rounds = (units + workers - 1) / workers;
-      const double t = rounds * ((pb + sk - 1) / sk) * stage_us + (sk > 1 ? (sk + 2) * dw_mb / 4.0 : 0.0);
-      if (t < best - 1e-9) best = t, s = sk;
-    }
-  } else {
-    const int mt = a->taps * ((a->c0 + 127) / 128 + (a->c1 + 127) / 128);
-    const int nt = (a->n + 255) / 256;
-    const int tiles = mt * nt;
-    // fill ~2 waves of 148 CTAs, keep >= 8 pixel blocks per split, bound the workspace
-    s = (2 * 148 + tiles - 1) / tiles;
-    if (s > pb / 8) s = pb / 8;
-    if (s < 1) s = 1;
-  }
+  const int mt = a->taps * ((a->c0 + 127) / 128 + (a->c1 + 127) / 128);
+  const int nt = a->n / 256 + (a->n % 256 != 0);
+  const int tiles = mt * nt;
+  // fill ~2 waves of CTAs, keep >= 8 pixel blocks per split, bound the workspace
+  int s = (2 * num_sms() + tiles - 1) / tiles;
+  if (s > pb / 8) s = pb / 8;
+  if (s < 1) s = 1;
   const int64_t wsz = static_cast<int64_t>(a->taps) * cin * a->n;
   while (s > 1 && wsz * s > (int64_t(48) << 20)) --s;  // <= 48M floats of partials
   *splits = s;
   *pblocks = pb;
   return 0;
+}
+
+template <int BN>
+static int wgrad_launch(WgradKArgs p, int n_begin, int nt, cudaStream_t stream) {
+  constexpr int SB = WG_A_BYTES + BN * 128;
+  p.n_begin = n_begin, p.NT = nt;
+  p.stages = WG_SMEM_BUDGET / SB;
+  if (p.stages > 8) p.stages = 8;
+  const size_t smem = (size_t)p.stages * SB + 256 + 1024;
+  static bool attr = false;
+  if (!attr) {
+    DDPO_CUDA_OK(cudaFuncSetAttribute(wgrad_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    attr = true;
+  }
+  const int tiles = p.splits * p.taps * (p.mt_per_tap0 + p.mt_per_tap1) * nt;
+  wgrad_kernel<BN><<<tiles, WG_THREADS, smem, stream>>>(p);
+  DDPO_LAUNCH_OK();
+  return DDPO_OK;
 }
 
 extern "C" int64_t ddpo_wgrad_workspace_floats(const ddpo_wgrad_args* a) {
@@ -299,6 +217,8 @@ extern "C" int ddpo_wgrad(const ddpo_wgrad_args* a, void* stream_) {
   DDPO_REQUIRE(a && a->dy && a->x0 && a->dw, "wgrad: null pointer");
   DDPO_REQUIRE(a->c0 % 64 == 0 && a->c1 % 64 == 0 && a->n % 64 == 0, "wgrad: channels must be multiples of 64");
   DDPO_REQUIRE(a->taps == 1 || a->taps == 9, "wgrad: taps must be 1 or 9");
+  DDPO_REQUIRE((reinterpret_cast<uintptr_t>(a->dw) & 7) == 0 && (reinterpret_cast<uintptr_t>(a->workspace) & 7) == 0,
+               "wgrad: dw and workspace must be 8-byte aligned (the epilogue stores column pairs)");
   WgradKArgs p;
   memset(&p, 0, sizeof(p));
   int splits, pblocks;
@@ -347,34 +267,23 @@ extern "C" int ddpo_wgrad(const ddpo_wgrad_args* a, void* stream_) {
     if (rc) return rc;
   }
   p.c0 = a->c0, p.c1 = a->c1, p.n = a->n, p.taps = a->taps, p.is_conv = a->is_conv;
-  p.pix_total = M, p.pblocks = pblocks, p.splits = splits;
+  p.pblocks = pblocks, p.splits = splits;
   p.pblocks_per_split = (pblocks + splits - 1) / splits;
   p.mt_per_tap0 = (a->c0 + 127) / 128, p.mt_per_tap1 = (a->c1 + 127) / 128;
   p.dst = splits > 1 ? a->workspace : a->dw;
   p.accumulate = 1;
-  if (wgrad_use_pair(a)) {
-    int rc = ddpo_wgrad2_launch(p.tmX0, p.tmX1, p.tmDY, a->c0, a->c1, a->n, a->taps, a->is_conv, p.W, p.H, p.conv_stride,
-                                splits, pblocks, p.dst, stream);
-    if (rc) return rc;
-  } else {
-    const int stage_bytes = WG_A_BYTES + 4 * WG_BOX_BYTES;
-    p.stages = WG_SMEM_BUDGET / stage_bytes;
-    const size_t smem = (size_t)p.stages * stage_bytes + 256 + 1024;
-    static bool attr = false;
-    if (!attr) {
-      DDPO_CUDA_OK(cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-      attr = true;
-    }
-    const int tiles = splits * p.taps * (p.mt_per_tap0 + p.mt_per_tap1) * ((a->n + 255) / 256);
-    int grid = num_sms();
-    if (grid > tiles) grid = tiles;
-    wgrad_kernel<<<grid, WG_THREADS, smem, stream>>>(p);
-    DDPO_LAUNCH_OK();
-  }
+  // 256-wide column tiles, then one launch for the remainder (64 / 128 / 192 columns)
+  const int n_main = a->n / 256 * 256, rem = a->n - n_main;
+  int rc = DDPO_OK;
+  if (n_main > 0 && (rc = wgrad_launch<256>(p, 0, n_main / 256, stream))) return rc;
+  if (rem == 64) rc = wgrad_launch<64>(p, n_main, 1, stream);
+  else if (rem == 128) rc = wgrad_launch<128>(p, n_main, 1, stream);
+  else if (rem == 192) rc = wgrad_launch<192>(p, n_main, 1, stream);
+  if (rc) return rc;
   if (splits > 1) {
     const int64_t n4 = static_cast<int64_t>(a->taps) * (a->c0 + a->c1) * a->n / 4;
     int blocks = static_cast<int>((n4 + 255) / 256);
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > num_sms() * 8) blocks = num_sms() * 8;
     wgrad_reduce_kernel<<<blocks, 256, 0, stream>>>(a->workspace, a->dw, n4, splits, 1);
     DDPO_LAUNCH_OK();
   }

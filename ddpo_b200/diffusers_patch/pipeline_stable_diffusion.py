@@ -5,7 +5,7 @@ classifier-free guidance and returns the whole trajectory plus per-step log-prob
 
     (final_latents [B,4,h,w], latents [B,T,4,h,w], next_latents [B,T,4,h,w], log_probs [B,T], ts [B,T])
 
-B200 design instead of ``pmap(lax.scan)``: one process per GPU owns its shard of the batch; one
+GPU design instead of ``pmap(lax.scan)``: one process per GPU owns its shard of the batch; one
 denoising step (U-Net on the 2B CFG batch + fused CFG/DDIM/log-prob/threefry kernel) is captured in
 a CUDA graph and replayed T times; the trajectory stays in HBM ([T+1, B, n] buffer, ``latents`` and
 ``next_latents`` are views of it).  Noise is bit-compatible with ``jax.random`` (same key lineage:

@@ -9,7 +9,7 @@ order, Python ``random`` prompts, the jax key lineage ``PRNGKey(seed) -> split -
 (``args.json``, ``samples/*.png``, ``rewards|prompts|callback_info|per_prompt_stats|train_info/*.npy``,
 ``checkpoints/checkpoint_<epoch>``).
 
-B200 design (SURVEY §8 a11/e):
+GPU design (SURVEY §8 a11/e):
   * one process per GPU (torchrun); a rank plays the role of one reference *worker* (``jax.process_index``) with one
     local device, so the per-worker batch permutation (:385-393) is already shard-local and no trajectory ever moves
     between GPUs; rewards / prompts are all-gathered exactly where the reference calls ``process_allgather``;

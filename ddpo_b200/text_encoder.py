@@ -8,9 +8,9 @@ host CPU "to save memory"; ``ddpo/training/diffusion.py:45-51,62-68`` inside the
 Parameter names / layouts are the Flax checkpoint's (``text_model/encoder/layers/<i>/self_attn/q_proj/kernel`` is
 ``[in, out]`` ...).  SD2 keeps 23 of ViT-H's 24 layers (the penultimate-layer conditioning is baked into the config).
 
-B200 design: 77-token sequences are tiny (4.5 GFLOP per prompt for SD2) -- the win is not the FLOPs but removing the
+GPU design: 77-token sequences are tiny (4.5 GFLOP per prompt for SD2) -- the win is not the FLOPs but removing the
 host-CPU stall and the H2D of the embeddings from every sample batch: q/k/v are one fused GEMM, attention is the U-Net's
-tcgen05 flash kernel with the causal bound added to its key mask, bias / residual ride in the GEMM epilogues."""
+wgmma flash kernel with the causal bound added to its key mask, bias / residual ride in the GEMM epilogues."""
 from dataclasses import dataclass
 from typing import Dict, List, Tuple
 

@@ -13,7 +13,7 @@ bucket datasets store them); the text side is either ``batch["input_ids"]`` / ``
 ``text_encoder`` callable exactly as the reference does (:47-51, :64-68), or -- when the caller has embedded the
 prompts already -- ``batch["prompt_embeds"]`` / ``batch["uncond_embeds"]``.
 
-B200 design: posterior sample, noise and ``add_noise`` are ONE kernel (jax-compatible threefry in registers); the
+GPU design: posterior sample, noise and ``add_noise`` are ONE kernel (jax-compatible threefry in registers); the
 conditional and unconditional U-Net applications run as one batch of 2B with context ``[uncond ; cond]``; the MSE on the
 CFG-combined prediction and its gradient are one kernel; forward + loss + backward replay as one CUDA graph; the
 ``lax.pmean(grad)`` (:96) is one NCCL all-reduce of the flat gradient folded into the fused clip+AdamW kernel.

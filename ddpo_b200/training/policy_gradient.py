@@ -11,7 +11,7 @@ Same call shape::
 ``prompt_embeds, uncond_embeds [B,77,D]`` (``pipeline/policy_gradient.py:415-423``); ``info`` has
 ``approx_kl, clipfrac, loss``.
 
-B200 design: the conditional and unconditional U-Net applications of ``compute_loss`` (:87-102) run as
+GPU design: the conditional and unconditional U-Net applications of ``compute_loss`` (:87-102) run as
 ONE batch of 2B with context ``[uncond ; cond]`` -- the very same kernels, tiles and reduction orders as
 the sampler, so on an unchanged policy ``ratio == 1`` bit-exactly.  Forward, fused log-prob, PPO loss and
 the whole backward are captured in one CUDA graph; weight gradients are accumulated straight into the

@@ -7,9 +7,9 @@ reference call sites ``ddpo/diffusers_patch/pipeline_flax_stable_diffusion.py:21
 ``ddpo_b200/unet_spec.py``.  This file only sequences kernel launches and owns buffers;
 all arithmetic happens in the CUDA library.
 
-Data flow design (B200-first):
+Data flow design:
   * the residual stream is fp32 NHWC; every GEMM/conv A operand is the bf16 output of the
-    preceding norm kernel; accumulation is fp32 in TMEM; bias / time-embedding / residual /
+    preceding norm kernel; accumulation is fp32 (wgmma register accumulators); bias / time-embedding / residual /
     GEGLU are fused in GEMM epilogues;
   * U-Net skip concatenations are never materialised (two-source norm + two-source conv);
   * cross-attention K/V projections depend only on the text context and are computed once per
@@ -99,8 +99,8 @@ class UNet:
         self.grads: Optional[torch.Tensor] = None  # flat fp32 gradient accumulator (same layout as params)
         self.train_mode = False
         # all ResNet time-embedding projections of a pass in ONE launch (ops.dense_small_grouped): bit-identical to the 22
-        # separate dense_small launches (tests/test_gpu_kernels.py), which cost ~36 us each at 10-40 CTAs -- measured
-        # 21.08 -> 20.62 ms per denoising step (profiles/README.md).  DDPO_GROUPED_TEMB=0 restores the separate launches.
+        # separate dense_small launches (tests/test_gpu_kernels.py), each of which runs only 10-40 CTAs.
+        # DDPO_GROUPED_TEMB=0 restores the separate launches.
         self.grouped_temb = os.environ.get("DDPO_GROUPED_TEMB", "1") == "1"
         self._temb_names = [n[: -len("/time_emb_proj/kernel")] for n in self.table if n.endswith("/time_emb_proj/kernel")]
         self._temb_tables: Dict[int, tuple] = {}

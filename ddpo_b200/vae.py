@@ -8,8 +8,8 @@ ResNets (+ nearest-2x upsample conv on the first 3), GroupNorm(32, eps 1e-6) + s
 Parameter names / layouts are the Flax checkpoint's (``decoder/...``, ``post_quant_conv``; ``kernel`` = HWIO / [in, out]);
 only the decoder half is held (the RWR path consumes stored posterior moments, it never encodes).
 
-B200 design: the same building blocks as the U-Net -- bf16 implicit-GEMM convolutions with fp32 TMEM accumulators
-(tcgen05), fused bias / residual epilogues, one-pass GroupNorm+swish (statistics from the producing GEMM's epilogue) writing the bf16
+GPU design: the same building blocks as the U-Net -- bf16 implicit-GEMM convolutions with fp32 accumulators
+(wgmma), fused bias / residual epilogues, one-pass GroupNorm+swish (statistics from the producing GEMM's epilogue) writing the bf16
 GEMM operand, fp32 residual stream.  Pixel rows at the 256 / 512 px levels are wider than a 128-row tile: the igemm TMA producer walks them as
 W/128 tiles per row.  The one attention layer has a single 512-wide head: scores are materialised per sample with two
 GEMMs around a row-softmax kernel (Q K^T -> softmax -> P V, V^T produced directly by a GEMM with swapped operands);

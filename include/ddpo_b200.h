@@ -1,4 +1,4 @@
-/* libddpo_b200 -- C ABI of the B200-native DDPO hot path.
+/* libddpo_b200 -- C ABI of the H100 (sm_90a) DDPO hot path.
  *
  * The reference (jannerm/ddpo) has no FFI layer: its seam is a set of Python call
  * signatures between pipeline/*.py and ddpo.* whose arithmetic runs inside XLA.  This
@@ -117,11 +117,11 @@ typedef struct {
   int ld_out;
   int geglu;                /* out_bf16[M, n/2] = lin * gelu_tanh(gate); weight rows tile-interleaved */
   int accumulate_out;       /* out_f32 += */
-  int bn_override;          /* 0 = auto */
+  int bn_override;          /* 0 = auto; else the tile width: 32, 64, 96, 128, 160, 192, 256 (320 = two 160 tiles) */
   void* aux_bf16;           /* GEGLU only, optional: bf16 [M, n] pre-activation (tile-interleaved, bias included) */
-  int mt_override;          /* 0 = auto; 1 / 2 = force 128- / 256-row CTA tiles */
-  int pair_override;        /* 0 = auto; 1 = force the CTA-pair (cta_group::2) kernel; 2 = force the 1-CTA kernel */
-  int epi_override;         /* 0 = auto; 1 = force the TMA-staged epilogue (pair kernel); 2 = force the register epilogue */
+  int mt_override;          /* scheduling hints kept for ABI compatibility; the sm_90a kernel has one tiling and one */
+  int pair_override;        /* epilogue, so these three are accepted and ignored (results never depend on them) */
+  int epi_override;
   int conv_pad;             /* 0 = the 3x3 default (symmetric pad 1); 1 = NO low-side padding: out[y,x] = sum in[s y + dy, s x + dx],
                                reads past the high edge are zero -- the VAE encoder's down-sample (pad ((0,1),(0,1)) + VALID) */
   float* gn_stats;          /* optional, with out_f32: fp32 [ceil(M/32), n, 2] = per 32-row slab and output column the (sum, sum
@@ -225,7 +225,7 @@ typedef struct {
   float* dw;       /* fp32 [taps*(c0+c1), n], accumulated */
   float* workspace;
   int64_t workspace_floats;
-  int kernel_override; /* 0 = auto (CTA-pair kernel, wgrad2.cu); 2 = force the 1-CTA kernel (wgrad.cu) */
+  int kernel_override; /* kept for ABI compatibility; ignored (one weight-gradient kernel) */
 } ddpo_wgrad_args;
 int64_t ddpo_wgrad_workspace_floats(const ddpo_wgrad_args* a);
 int ddpo_wgrad(const ddpo_wgrad_args* a, void* stream);

@@ -2,9 +2,8 @@
 encode of 8 prompts (SD2 tower), the RWR input/loss kernels and the trajectory gather -- bracketed by
 cudaProfilerStart/Stop after a warm-up pass.
 
-    ncu --profile-from-start off --clock-control none --csv --log-file gpurun_out/launches_aux.csv \
-        --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum python tests/prof_aux.py
-    python profiles/make_launch_summary.py --out r1_aux_launches aux=gpurun_out/launches_aux.csv
+    ncu --profile-from-start off --csv --metrics gpu__time_duration.sum,dram__bytes_read.sum,dram__bytes_write.sum \
+        python tests/prof_aux.py
 """
 import os
 import sys

@@ -114,7 +114,7 @@ def ln_bwd(m, c):
     print(f"ln_bwd M{m} C{c}: {t * 1e6:8.1f} us  {alg / t / 1e9:7.0f} GB/s algorithmic ({alg / t / 1e9 / PEAK:.2f})")
 
 
-gn_fwd(16, 4096, 320, 0)            # the dominant sampling shape (profiles/r1_gn.md)
+gn_fwd(16, 4096, 320, 0)            # the dominant sampling shape
 gn_fwd(16, 4096, 320, 0, with_stats=False, tag="[two-pass]")
 if not once:
     os.environ["DDPO_GN_STREAM"] = "1"

@@ -12,7 +12,7 @@ def bf(x):
     return x.to(torch.bfloat16)
 
 
-@pytest.mark.parametrize("kernel", [0, 2])  # 0 = CTA-pair kernel (wgrad2.cu), 2 = 1-CTA kernel (wgrad.cu)
+@pytest.mark.parametrize("kernel", [0, 2])  # kernel_override: a hint the library ignores
 @pytest.mark.parametrize("m,k,n", [(256, 64, 64), (1000, 320, 320), (4096, 1280, 640), (154, 1024, 1280), (8192, 128, 960),
                                    (5000, 192, 192), (40960, 320, 2560)])
 def test_wgrad_linear(m, k, n, kernel):

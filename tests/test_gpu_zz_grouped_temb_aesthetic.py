@@ -1,6 +1,5 @@
-"""Paths that round 1 shipped without a GPU run; all of them ran green on a B200 in round 2 (gpurun call 1) and are part of
-the regular suite now: the grouped time-embedding projection launch (bit-identical to the separate launches; default ON
-since it measured 21.08 -> 20.62 ms per denoising step) and the aesthetic reward model on the GPU kernels (CLIP ViT image
+"""The grouped time-embedding projection launch (bit-identical to the separate launches; default ON: one launch instead
+of one per ResNet block) and the aesthetic reward model on the GPU kernels (CLIP ViT image
 tower + LAION head against the oracle pinned to `transformers`)."""
 import os
 
