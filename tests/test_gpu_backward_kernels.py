@@ -56,7 +56,10 @@ def test_wgrad_conv(b, h, c0, c1, n, ks, stride, kernel):
 
 
 @pytest.mark.parametrize("dy_dtype", [torch.float32, torch.bfloat16])
-@pytest.mark.parametrize("b,hw,c0,c1,silu", [(2, 64, 64, 0, True), (2, 1024, 320, 0, True), (2, 256, 128, 64, False)])
+@pytest.mark.parametrize("b,hw,c0,c1,silu", [(2, 64, 64, 0, True), (2, 1024, 320, 0, True), (2, 256, 128, 64, False),
+                                             # SD2-base up-block resnets: cin = 2560, 1920, 960, 640
+                                             (2, 64, 1280, 1280, True), (2, 256, 1280, 640, True),
+                                             (2, 1024, 640, 320, True), (2, 4096, 320, 320, True)])
 def test_groupnorm_bwd(b, hw, c0, c1, silu, dy_dtype):
     from ddpo_b200 import ops
     g = torch.Generator(device="cpu").manual_seed(2)
