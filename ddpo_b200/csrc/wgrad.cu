@@ -217,8 +217,8 @@ extern "C" int ddpo_wgrad(const ddpo_wgrad_args* a, void* stream_) {
   DDPO_REQUIRE(a && a->dy && a->x0 && a->dw, "wgrad: null pointer");
   DDPO_REQUIRE(a->c0 % 64 == 0 && a->c1 % 64 == 0 && a->n % 64 == 0, "wgrad: channels must be multiples of 64");
   DDPO_REQUIRE(a->taps == 1 || a->taps == 9, "wgrad: taps must be 1 or 9");
-  DDPO_REQUIRE((reinterpret_cast<uintptr_t>(a->dw) & 7) == 0 && (reinterpret_cast<uintptr_t>(a->workspace) & 7) == 0,
-               "wgrad: dw and workspace must be 8-byte aligned (the epilogue stores column pairs)");
+  DDPO_REQUIRE((reinterpret_cast<uintptr_t>(a->dw) & 15) == 0 && (reinterpret_cast<uintptr_t>(a->workspace) & 15) == 0,
+               "wgrad: dw and workspace must be 16-byte aligned (the split reduction loads and stores float4)");
   WgradKArgs p;
   memset(&p, 0, sizeof(p));
   int splits, pblocks;

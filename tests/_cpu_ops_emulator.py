@@ -609,6 +609,8 @@ def grad_sumsq(g, ws, out):
 
 
 def clip_adamw(params, grad_acc, mu, nu, sumsq, grad_scale, max_norm, lr, b1, b2, eps, wd, step, norm_out=None):
+    # the kernel receives the hyperparameters as fp32 and forms 1 - b1 and 1 - b2 from those (exact in fp32)
+    lr, b1, b2, eps, wd = (float(np.float32(v)) for v in (lr, b1, b2, eps, wd))
     norm = float(grad_scale) * float(sumsq.sqrt())
     g = grad_acc * float(grad_scale)
     if not norm < max_norm:

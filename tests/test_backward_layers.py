@@ -21,116 +21,8 @@ margins of the bounds below are on record.
 import pytest
 import torch
 import torch.nn.functional as F
-
-BF16, F32, F64 = torch.bfloat16, torch.float32, torch.float64
-
-# Bounds.  The worst errors of the CUDA kernels over all cases below, measured on an H100 80GB HBM3 (700 W), are in the
-# comments.  The fp32, bf16-L2 and attention-L2 bounds are the rest of the suite's, not fitted to these numbers.
-F32_MAX, F32_L2 = 2e-3, 1e-3          # fp32 outputs (fp32 accumulation of bf16 operands): worst 1.6e-5, 1.3e-5
-BF16_MAX, BF16_L2 = 8e-3, 4e-3        # bf16 outputs, whose rounding alone is up to 2^-8 of the value: worst 3.5e-3, 1.7e-3
-ATT_MAX, ATT_L2 = 2e-2, 2e-2          # attention gradients (P and dS pass through bf16): worst 4.7e-3, 2.8e-3
-SUM_TOL = 1e-5                        # reductions, in units of sum |term|: worst 0.33 of the bound (dense_small dW)
-F32_ULP = 2.0 ** -23                  # one fp32 rounding of an accumulate-into (out = old + sum)
-
-
-# --------------------------------------------------------------------------------------------------- harness ------
-class Backend:
-    """The ops module a check runs on: the CUDA library, or its torch-CPU emulation."""
-
-    def __init__(self, name):
-        self.emulated = name == "emulator"
-        if self.emulated:
-            import _cpu_ops_emulator as ops
-            self.dev = "cpu"
-        else:
-            from ddpo_b200 import ops
-            self.dev = "cuda"
-        self.ops = ops
-        # extra columns past the pitch for ops that take a row pitch; the emulator writes dense outputs (it has no
-        # ld_out), so its outputs get extra rows only
-        self.pad = 0 if self.emulated else 64
-
-    def sync(self):
-        if not self.emulated:
-            torch.cuda.synchronize()
-
-
-def _backend_params(small, large=()):
-    """(backend, *case) parameter sets: small cases on both backends, large ones on the GPU only"""
-    out = []
-    for case in small:
-        out.append(pytest.param("emulator", *case, id="emu-" + "-".join(map(str, case))))
-    for case in list(small) + list(large):
-        out.append(pytest.param("cuda", *case, marks=pytest.mark.gpu, id="cuda-" + "-".join(map(str, case))))
-    return out
-
-
-_NODE = {}
-
-
-@pytest.fixture(autouse=True)
-def _current_node(request):
-    _NODE["node"] = request.node
-    yield
-    _NODE.pop("node", None)
-
-
-def _record(name, **vals):
-    node = _NODE.get("node")
-    if node is not None:
-        node.user_properties.append((name, " ".join(f"{k}={v:.3g}" for k, v in vals.items())))
-
-
-class Guarded:
-    """A [rows, cols] output at the top-left of a larger buffer: ``extra_cols`` past the pitch, ``extra_rows`` after the
-    last row.  The buffer starts as seeded noise (``init`` goes into the view) and everything outside the view must
-    come back unchanged (``check``)."""
-
-    def __init__(self, rows, cols, dtype, dev, extra_cols=0, extra_rows=8, init=None, seed=99):
-        g = torch.Generator().manual_seed(seed)
-        self.buf = (torch.randn(rows + extra_rows, cols + extra_cols, generator=g) * 1e3 + 4097.0).to(dtype).to(dev)
-        self.rows, self.cols, self.ld = rows, cols, cols + extra_cols
-        if init is not None:
-            self.view.copy_(init.reshape(rows, cols))
-        self.snapshot = self.buf.clone()
-
-    @property
-    def view(self):
-        return self.buf[:self.rows, :self.cols]
-
-    @property
-    def arg(self):
-        """what to hand to an op: the dense view where there are no extra columns, else the whole pitched buffer"""
-        return self.view if self.ld == self.cols else self.buf
-
-    def check(self, what):
-        outside = torch.ones(self.buf.shape, dtype=torch.bool, device=self.buf.device)
-        outside[:self.rows, :self.cols] = False
-        assert torch.equal(self.buf[outside], self.snapshot[outside]), f"{what}: write outside the output"
-
-
-def check_close(name, out, ref, max_tol, l2_tol):
-    d = out.double() - ref
-    rmax = ref.abs().max().item()
-    e_max = d.abs().max().item() / rmax
-    e_l2 = (d.norm() / ref.norm()).item()
-    _record(name, max=e_max, l2=e_l2)
-    assert e_max <= max_tol and e_l2 <= l2_tol, \
-        f"{name}: max err {e_max:.3g} * max|ref| (bound {max_tol}), relative L2 {e_l2:.3g} (bound {l2_tol})"
-
-
-def check_sum(name, out, ref, abs_terms, tol=SUM_TOL, old=None):
-    """out (+)= a sum: |out - old - ref| <= tol * sum|terms| (+ one rounding of the add into ``old``)"""
-    o = out.double()
-    err = (o - (old.double() if old is not None else 0) - ref).abs()
-    bound = tol * abs_terms + (2 * F32_ULP * o.abs() if old is not None else 0) + 1e-30
-    worst = (err / bound).max().item()
-    _record(name, worst_over_bound=worst, rel_to_abs_sum=(err / (abs_terms + 1e-30)).max().item())
-    assert worst <= 1.0, f"{name}: error {worst:.3g} x the bound ({tol} * sum|terms|)"
-
-
-def rnd(g, *shape, scale=1.0, shift=0.0):
-    return torch.randn(*shape, generator=g) * scale + shift
+from _layer_check import (ATT_L2, ATT_MAX, BF16, BF16_L2, BF16_MAX, F32, F32_L2, F32_MAX, F64, SUM_TOL, Backend,
+                          Guarded, _backend_params, _current_node, _record, check_close, check_sum, rnd)  # noqa: F401
 
 
 def hwio_to_oihw(w):
