@@ -25,7 +25,7 @@ class IGemmArgs(C.Structure):
                 ("is_conv", i32), ("batch", i32), ("h", i32), ("w", i32), ("conv_stride", i32), ("taps", i32),
                 ("m", i32), ("n", i32), ("wt", vp), ("bias", vp), ("rowvec", vp), ("rows_per_sample", i32),
                 ("rowvec_ld", i32), ("residual", vp), ("ld_res", i32), ("out_f32", vp), ("out_bf16", vp),
-                ("ld_out", i32), ("geglu", i32), ("accumulate_out", i32), ("bn_override", i32), ("aux_bf16", vp), ("mt_override", i32), ("pair_override", i32), ("epi_override", i32),
+                ("ld_out", i32), ("geglu", i32), ("accumulate_out", i32), ("bn_override", i32), ("aux_bf16", vp),
                 ("conv_pad", i32), ("gn_stats", vp)]
 
 
@@ -46,14 +46,14 @@ class WgradArgs(C.Structure):
     _fields_ = [("dy", vp), ("ldy", i32), ("n", i32), ("x0", vp), ("x1", vp), ("c0", i32), ("c1", i32),
                 ("ldx0", i32), ("ldx1", i32), ("is_conv", i32), ("batch", i32), ("h", i32), ("w", i32),
                 ("conv_stride", i32), ("taps", i32), ("m", i32), ("dw", vp), ("workspace", vp),
-                ("workspace_floats", i64), ("kernel_override", i32)]
+                ("workspace_floats", i64)]
 
 
 class AttentionBwdArgs(C.Structure):
     _fields_ = [("q", vp), ("k", vp), ("v", vp), ("out", vp), ("dout", vp), ("lse", vp), ("delta", vp),
                 ("dq", vp), ("dk", vp), ("dv", vp), ("batch", i32), ("heads", i32), ("nq", i32), ("nk", i32),
                 ("head_dim", i32), ("ldq", i32), ("ldk", i32), ("ldv", i32), ("ldo", i32), ("lddo", i32),
-                ("lddq", i32), ("lddk", i32), ("lddv", i32), ("workspace", vp)]
+                ("lddq", i32), ("lddk", i32), ("lddv", i32)]
 
 
 # name -> (restype, argtypes).  Every symbol declared in include/ddpo_b200.h is listed here;

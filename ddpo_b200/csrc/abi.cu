@@ -102,4 +102,4 @@ extern "C" int ddpo_device_sm_count(void) {
   }
   return n;
 }
-extern "C" int ddpo_abi_version(void) { return 2; }
+extern "C" int ddpo_abi_version(void) { return 3; }

@@ -144,7 +144,7 @@ __global__ void __launch_bounds__(AB_THREADS, 1) attention_bwd_dkdv_kernel(const
         for (int e = 0; e < 2; ++e) {
           const int x = 4 * j + 2 * h + e, col = 8 * j + 2 * t4 + e;
           const bool ok = key_ok[h] && i * 64 + col < p.nq;
-          const float pr = ok ? ex2_sel<DDPO_EXP_POLY_BWD>(col, fmaf(s[x], p.scale_log2e, -lse_l2[2 * j + e])) : 0.f;
+          const float pr = ok ? ex2_mufu(fmaf(s[x], p.scale_log2e, -lse_l2[2 * j + e])) : 0.f;
           s[x] = pr;
           dp[x] = pr * fmaf(dp[x], p.scale, -delta_s[2 * j + e]);
         }
@@ -255,7 +255,7 @@ __global__ void __launch_bounds__(AB_THREADS, 1) attention_bwd_dq_kernel(const _
         for (int e = 0; e < 2; ++e) {
           const int x = 4 * jj + 2 * h + e, col = 8 * jj + 2 * t4 + e;
           const bool ok = row_ok[h] && col < valid_keys;
-          const float pr = ok ? ex2_sel<DDPO_EXP_POLY_BWD>(col, fmaf(s[x], p.scale_log2e, -lse_l2[h])) : 0.f;
+          const float pr = ok ? ex2_mufu(fmaf(s[x], p.scale_log2e, -lse_l2[h])) : 0.f;
           dp[x] = pr * fmaf(dp[x], p.scale, -delta_s[h]);
         }
     uint32_t da[4][4];

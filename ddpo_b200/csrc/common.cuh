@@ -42,7 +42,6 @@ int make_tensor_map(CUtensorMap* out, const void* base, int elem_bytes, int rank
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
-__device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -59,7 +58,7 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
 }
 __device__ __forceinline__ float bf16_lo(uint32_t v) { return __uint_as_float(v << 16); }
 __device__ __forceinline__ float bf16_hi(uint32_t v) { return __uint_as_float(v & 0xffff0000u); }
-__device__ __forceinline__ float exp2f_approx(float x) {
+__device__ __forceinline__ float ex2_mufu(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
@@ -71,7 +70,7 @@ __device__ __forceinline__ float rcpf_approx(float x) {
 }
 // sigmoid / SiLU on the two MUFU ops ex2 + rcp (relative error ~2e-7); the IEEE division of x / (1 + __expf(-x)) cost
 // ~10 more instructions per element in the GroupNorm apply kernels, which are issue- as much as bandwidth-limited.
-__device__ __forceinline__ float sigmoid_f(float x) { return rcpf_approx(1.0f + exp2f_approx(-1.4426950408889634f * x)); }
+__device__ __forceinline__ float sigmoid_f(float x) { return rcpf_approx(1.0f + ex2_mufu(-1.4426950408889634f * x)); }
 __device__ __forceinline__ float silu_f(float x) { return x * sigmoid_f(x); }
 // SiLU on ONE MUFU op: x sigmoid(x) = z + z tanh(z), z = x / 2 (tanh.approx: max relative error 2^-11, an order below
 // bf16 resolution).  Used where the result is rounded to bf16 anyway (the GroupNorm -> GEMM-operand path, which is
@@ -87,28 +86,23 @@ __device__ __forceinline__ float gelu_tanh_f(float x) {
   float u = k * (x + 0.044715f * x * x * x);
   // 0.5 (1 + tanh u) == 1 / (1 + e^{-2u}): two MUFU ops (ex2, rcp) instead of libm tanhf's ~25 instructions;
   // relative error ~2e-7, exact limits at +-inf
-  const float e = exp2f_approx(-2.885390081777927f * u);  // e^{-2u}
+  const float e = ex2_mufu(-2.885390081777927f * u);  // e^{-2u}
   return x * rcpf_approx(1.0f + e);
 }
 __device__ __forceinline__ float gelu_tanh_grad_f(float x) {
   const float k = 0.7978845608028654f;
   float u = k * (x + 0.044715f * x * x * x);
-  const float e = exp2f_approx(fminf(-2.885390081777927f * u, 80.0f));  // e^{-2u}, clamped so that e * sg stays finite
+  const float e = ex2_mufu(fminf(-2.885390081777927f * u, 80.0f));  // e^{-2u}, clamped so that e * sg stays finite
   const float sg = rcpf_approx(1.0f + e);  // (1 + tanh u) / 2
   float du = k * (1.0f + 3.0f * 0.044715f * x * x);
   // d/dx [x sg] with 1 - tanh^2 u = 4 e sg^2 (no cancellation near |tanh| = 1)
   return sg + 2.0f * x * du * (e * sg) * sg;
 }
 
-// 2^x for x <= 0 two ways: the MUFU unit (16/clk/SM) and a Cody-Waite + degree-3 polynomial on the FMA/ALU pipes
-// (max relative error 8.8e-5, far below bf16 resolution).  The attention kernels alternate them by COLUMN
+// 2^x for x <= 0 on the FMA/ALU pipes instead of the MUFU unit (16/clk/SM): Cody-Waite + degree-3 polynomial
+// (max relative error 8.8e-5, far below bf16 resolution).  The attention forward alternates it with ex2_mufu by COLUMN
 // PARITY (a fixed function of the element position -> deterministic, batch-invariant) because the softmax
 // exponentials, not the tensor cores, bound the kernel when every element goes through MUFU.
-__device__ __forceinline__ float ex2_mufu(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
 __device__ __forceinline__ float ex2_poly(float x) {
   x = fmaxf(x, -126.0f);
   const float r = __fadd_rd(x, 12582912.0f);  // 1.5 * 2^23: low mantissa bits now hold floor(x)
@@ -117,15 +111,12 @@ __device__ __forceinline__ float ex2_poly(float x) {
   return __int_as_float(__float_as_int(p) + ((__float_as_int(r) - 0x4B400000) << 23));
 }
 
-// Which columns of a 32-wide chunk take the polynomial: every DDPO_EXP_POLY_{FWD,BWD}-th one (0 = none).  The split
+// Which columns of a 32-wide chunk take the polynomial: every DDPO_EXP_POLY_FWD-th one (0 = none).  The split
 // is a fixed function of the element's position, so results stay deterministic and batch invariant.
 // The polynomial costs ~10 issue slots against 1 for MUFU.EX2, so only the forward kernel (fewer other instructions
-// per score) keeps a small share.
+// per score) keeps a small share; the backward uses MUFU alone.
 #ifndef DDPO_EXP_POLY_FWD
 #define DDPO_EXP_POLY_FWD 8
-#endif
-#ifndef DDPO_EXP_POLY_BWD
-#define DDPO_EXP_POLY_BWD 0
 #endif
 template <int PERIOD>
 __device__ __forceinline__ float ex2_sel(int i, float x) {
@@ -139,9 +130,6 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 }
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void fence_proxy_async_smem() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
@@ -168,17 +156,6 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 #ifndef DDPO_MBAR_TIMEOUT_CYCLES
 #define DDPO_MBAR_TIMEOUT_CYCLES 8000000000ll  // ~4 s at 2 GHz
 #endif
-__device__ __forceinline__ bool mbar_try_wait_hint(uint64_t* bar, uint32_t parity, uint32_t hint_ns) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 P, [%1], %2, %3;\n\t"
-      "selp.b32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity), "r"(hint_ns)
-      : "memory");
-  return ok != 0;
-}
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   long long t0 = 0;
@@ -193,10 +170,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 
 // -------------------------------------------------------------------- TMA ----
-// pull the 128-byte line holding `ptr` into L2 (no register, no scoreboard entry)
-__device__ __forceinline__ void prefetch_l2(const void* ptr) {
-  asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<uint64_t>(ptr)));
-}
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
 }
@@ -214,29 +187,6 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-
-// 1-D bulk copy global -> shared (no tensor map): `bytes` contiguous bytes, 16-byte aligned on both sides, completion
-// credited to an mbarrier like a tensor load
-__device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   smem_u32(smem_dst)),
-               "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMA store (shared -> global, bulk async-group completion); rows/columns outside the tensor are clipped
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_read() {  // all but the N most recent groups have finished READING smem
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // ------------------------------------------------------------------ wgmma ----
 // Shared-memory matrix descriptor of a SWIZZLE_128B operand (sm_90): start address, leading and stride byte offsets

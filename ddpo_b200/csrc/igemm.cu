@@ -285,8 +285,7 @@ extern "C" int ddpo_igemm(const ddpo_igemm_args* a, void* stream_) {
   DDPO_REQUIRE(a->taps == 1 || a->taps == 9, "ddpo_igemm: taps must be 1 or 9");
   DDPO_REQUIRE(a->n % 32 == 0, "ddpo_igemm: N=%d must be a multiple of 32", a->n);
   DDPO_REQUIRE(a->out_f32 != nullptr || a->out_bf16 != nullptr, "ddpo_igemm: no output");
-  int BN = a->bn_override > 0 ? a->bn_override : pick_width(a->n, a->geglu);
-  if (BN == 320 && !a->geglu) BN = 160;  // a 320-wide tile is two 160-column tiles
+  const int BN = a->bn_override > 0 ? a->bn_override : pick_width(a->n, a->geglu);
   DDPO_REQUIRE(BN == 32 || BN == 64 || BN == 96 || BN == 128 || BN == 160 || BN == 192 || BN == 256,
                "ddpo_igemm: unsupported tile width %d", BN);
   DDPO_REQUIRE(a->n % BN == 0, "ddpo_igemm: no valid BN for N=%d", a->n);

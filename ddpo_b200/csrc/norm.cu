@@ -17,12 +17,9 @@
 // gn_finalize_chunks_kernel.  Either way the reduction order depends on (HW, C) only, never on the batch size ->
 // batch-invariant, bit-reproducible results.
 //
-// Apply.  gn_apply_tma_kernel streams x through a 4-stage shared-memory ring filled by 1-D bulk copies (one producer
-// thread keeps ~100 KB per CTA in flight whatever the occupancy), consumer threads own a fixed channel quad (scale, bias,
-// mean, rstd in registers) and write 8-byte bf16 pieces of consecutive channels; work is a flat list of (sample, pixel
-// range) stages split evenly over 2 CTAs per SM -> one wave, no tail.
+// Apply.  gn_apply_kernel runs on the same (pixel chunk, sample) grid as gn_stats_kernel: a thread owns a channel quad
+// (the per-channel affine coefficients in registers) and keeps four independent 16-byte loads of x in flight.
 #include "common.cuh"
-#include <stdlib.h>
 
 #include "reduce.cuh"
 
@@ -174,10 +171,10 @@ __global__ void gn_finalize_chunks_kernel(const GnArgs a, int batch) {
   a.mr[i * 2] = mean, a.mr[i * 2 + 1] = rsqrtf(var + a.eps);
 }
 
-// Per-element arithmetic shared by the two apply kernels (bit-identical outputs whichever runs): the affine part as ONE
-// fused multiply-add y = x * A + B with A = rstd * scale, B = bias - mean * A (per thread and channel, computed once), SiLU
-// on one MUFU op when the only consumer is the bf16 GEMM operand.  The apply pass was issue- / MUFU-bound with the
-// three-instruction affine and the two-MUFU sigmoid.
+// Per-element arithmetic of the apply kernel: the affine part as ONE fused multiply-add y = x * A + B with
+// A = rstd * scale, B = bias - mean * A (per thread and channel, computed once), SiLU on one MUFU op when the only
+// consumer is the bf16 GEMM operand.  The apply pass was issue- / MUFU-bound with the three-instruction affine and the
+// two-MUFU sigmoid.
 __device__ __forceinline__ void gn_coef(float mean, float rstd, float scale, float bias, float& A, float& B) {
   A = rstd * scale;
   B = fmaf(-mean, A, bias);
@@ -187,102 +184,6 @@ __device__ __forceinline__ float gn_act(float x, float A, float B, int silu) {
   const float y = fmaf(x, A, B);
   if (!silu) return y;
   return FAST ? silu_bf16_f(y) : silu_f(y);
-}
-
-// ------------------------------------------------------------ streamed apply (forward) ----
-constexpr int GNA_STAGES = 4;
-constexpr int GNA_STAGE_BYTES = 24 * 1024;
-
-struct GnStream {
-  int c4[2];        // channel quads per source
-  int pix[2];       // pixels per stage per source (power of two dividing hw)
-  int ctas[2];      // CTAs working on each source (blockIdx.z = source)
-  int consumers;    // consumer threads (block = 32 + consumers)
-};
-
-__global__ void __launch_bounds__(544, 1) gn_apply_tma_kernel(const GnArgs a, const GnStream g, int batch) {
-  extern __shared__ __align__(128) uint8_t gna_smem[];
-  const int src = blockIdx.z;
-  if (static_cast<int>(blockIdx.x) >= (src == 0 ? g.ctas[0] : g.ctas[1])) return;
-  uint64_t* full = reinterpret_cast<uint64_t*>(gna_smem + GNA_STAGES * GNA_STAGE_BYTES);
-  uint64_t* empty = full + GNA_STAGES;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_cwarps = (g.consumers + 31) >> 5;
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < GNA_STAGES; ++i) mbar_init(&full[i], 1), mbar_init(&empty[i], n_cwarps);
-    fence_barrier_init();
-  }
-  __syncthreads();
-  const int C = a.c0 + a.c1, cpg = C / GN_GROUPS;
-  const int cs = src == 0 ? a.c0 : a.c1, coff = src == 0 ? 0 : a.c0;
-  const float* x = src == 0 ? a.x0 : a.x1;
-  const int P = src == 0 ? g.pix[0] : g.pix[1];
-  const int n_ctas = src == 0 ? g.ctas[0] : g.ctas[1];
-  const int spp = a.hw / P;                                // stages per sample
-  const long total = static_cast<long>(batch) * spp;      // flat stage list of this source
-  const long per = (total + n_ctas - 1) / n_ctas;
-  const long it0 = per * blockIdx.x, it1 = it0 + per < total ? it0 + per : total;
-  const uint32_t stage_bytes = static_cast<uint32_t>(P) * cs * 4;
-  if (warp == 0) {
-    if (lane == 0) {
-      for (long it = it0; it < it1; ++it) {
-        const int k = static_cast<int>(it - it0), st = k % GNA_STAGES;
-        mbar_wait(&empty[st], ((k / GNA_STAGES) & 1) ^ 1);
-        mbar_expect_tx(&full[st], stage_bytes);
-        bulk_load_1d(gna_smem + st * GNA_STAGE_BYTES, x + static_cast<size_t>(it) * P * cs, stage_bytes, &full[st]);
-      }
-    }
-    return;
-  }
-  const int ct = threadIdx.x - 32;
-  const int C4 = src == 0 ? g.c4[0] : g.c4[1], R = g.consumers / C4;
-  const int cq = ct % C4, pr = ct / C4;
-  const bool active = ct < R * C4;
-  const int c = coff + cq * 4;
-  float scv[4], biv[4], cA[4], cB[4];
-  {
-    const float4 sc = *reinterpret_cast<const float4*>(a.scale + c), bi = *reinterpret_cast<const float4*>(a.bias + c);
-    scv[0] = sc.x, scv[1] = sc.y, scv[2] = sc.z, scv[3] = sc.w;
-    biv[0] = bi.x, biv[1] = bi.y, biv[2] = bi.z, biv[3] = bi.w;
-  }
-  const bool fast = a.y_f32 == nullptr;   // only the bf16 operand is written: one-MUFU SiLU
-  int cur_b = -1;
-  for (long it = it0; it < it1; ++it) {
-    const int k = static_cast<int>(it - it0), st = k % GNA_STAGES;
-    const int b = static_cast<int>(it / spp);
-    const size_t pix0 = static_cast<size_t>(it) * P;      // global pixel index (b * hw + p)
-    if (b != cur_b) {
-      cur_b = b;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 m = *reinterpret_cast<const float2*>(a.mr + (b * GN_GROUPS + (c + j) / cpg) * 2);
-        gn_coef(m.x, m.y, scv[j], biv[j], cA[j], cB[j]);
-      }
-    }
-    mbar_wait(&full[st], (k / GNA_STAGES) & 1);
-    if (active) {
-      const float4* sm4 = reinterpret_cast<const float4*>(gna_smem + st * GNA_STAGE_BYTES);
-      for (int pp = pr; pp < P; pp += R) {
-        const float4 v = sm4[pp * C4 + cq];
-        const float xv[4] = {v.x, v.y, v.z, v.w};
-        float y[4];
-        if (fast) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) y[j] = gn_act<true>(xv[j], cA[j], cB[j], a.silu);
-        } else {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) y[j] = gn_act<false>(xv[j], cA[j], cB[j], a.silu);
-        }
-        const size_t o = (pix0 + pp) * C + c;
-        if (a.y_bf16) *reinterpret_cast<uint2*>(a.y_bf16 + o) = make_uint2(pack_bf16(y[0], y[1]), pack_bf16(y[2], y[3]));
-        if (a.y_f32) *reinterpret_cast<float4*>(a.y_f32 + o) = make_float4(y[0], y[1], y[2], y[3]);
-        if (a.raw_bf16)
-          *reinterpret_cast<uint2*>(a.raw_bf16 + o) = make_uint2(pack_bf16(xv[0], xv[1]), pack_bf16(xv[2], xv[3]));
-      }
-    }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[st]);
-  }
 }
 
 __global__ void __launch_bounds__(GN_THREADS) gn_apply_kernel(const GnArgs a) {
@@ -352,8 +253,6 @@ struct GnBwdArgs {
   int ldd0, ldd1;
   int accumulate;
   float* dparam_part;  // [B, chunks, 2, C]  partial (dscale, dbias)
-  int b0;              // first sample of this launch: the two passes run over groups of samples small enough that the
-                       // second pass finds x and dy in L2 (126 MB) instead of fetching them from DRAM again
 };
 
 // four consecutive gradient values at element index `idx` (a multiple of 4).  The element type is a TEMPLATE parameter of
@@ -381,7 +280,7 @@ __global__ void __launch_bounds__(GN_THREADS) gn_bwd_stats_kernel(const GnBwdArg
   const int cols = C4 < GN_THREADS ? C4 : GN_THREADS;
   const int R = GN_THREADS / cols;
   const int tc = threadIdx.x % cols, tr = threadIdx.x / cols;
-  const int b = a.b0 + blockIdx.y, chunk = blockIdx.x;
+  const int b = blockIdx.y, chunk = blockIdx.x;
   const int p_begin = chunk * f.pix_per_chunk;
   const int p_end = min(f.hw, p_begin + f.pix_per_chunk);
   extern __shared__ float sm[];  // [R][C][4] : a0, a1, dscale, dbias per channel
@@ -458,8 +357,8 @@ __global__ void __launch_bounds__(GN_THREADS, 2) gn_bwd_apply_kernel(const GnBwd
   const int cols = C4 < GN_THREADS ? C4 : GN_THREADS;
   const int R = GN_THREADS / cols;
   const int tc = threadIdx.x % cols, tr = threadIdx.x / cols;
-  // descending order within the launch: the stats pass finished on the last samples / chunks, start with those
-  const int b = a.b0 + (gridDim.y - 1 - blockIdx.y), chunk = gridDim.x - 1 - blockIdx.x;
+  // descending order: the stats pass finished on the last samples / chunks, start with those
+  const int b = gridDim.y - 1 - blockIdx.y, chunk = gridDim.x - 1 - blockIdx.x;
   const int p_begin = chunk * f.pix_per_chunk;
   const int p_end = min(f.hw, p_begin + f.pix_per_chunk);
   __shared__ float s_mean[GN_GROUPS], s_rstd[GN_GROUPS], s_m1[GN_GROUPS], s_m2[GN_GROUPS];
@@ -727,55 +626,6 @@ extern "C" int64_t ddpo_groupnorm_workspace_floats(int batch, int hw, int channe
          static_cast<int64_t>(batch) * chunks * 2 * channels;
 }
 
-// plan of the streamed apply pass; returns false when the shape does not fit it (the two-pass kernels then run)
-static bool gn_stream_plan(const GnArgs& g, const ddpo_groupnorm_args* a, GnStream* st) {
-  // Opt-in ($DDPO_GN_STREAM=1; read per call: the bit-identity test toggles it).  The plain kernel (every thread issuing
-  // its own 16-byte loads) is the default; this TMA-staged one is kept as a developer A/B switch.
-  const char* on = getenv("DDPO_GN_STREAM");
-  if (on == nullptr || on[0] != '1') return false;
-  const int nsrc = a->c1 > 0 ? 2 : 1;
-  if (g.ld0 != a->c0 || (nsrc == 2 && g.ld1 != a->c1)) return false;          // sources must be dense (1-D bulk copies)
-  if ((reinterpret_cast<uintptr_t>(a->x0) & 15) || (nsrc == 2 && (reinterpret_cast<uintptr_t>(a->x1) & 15))) return false;
-  if (a->c0 % 4 != 0 || a->c1 % 4 != 0 || (a->hw & (a->hw - 1)) != 0) return false;
-  long bytes[2] = {0, 0};
-  for (int s = 0; s < nsrc; ++s) {
-    const int cs = s == 0 ? a->c0 : a->c1;
-    st->c4[s] = cs / 4;
-    if (st->c4[s] > 512) return false;
-    int pix = 1;
-    while (pix * 2 <= a->hw && static_cast<long>(pix) * 2 * cs * 4 <= GNA_STAGE_BYTES) pix *= 2;
-    if (static_cast<long>(pix) * cs * 4 > GNA_STAGE_BYTES) return false;
-    st->pix[s] = pix;
-    bytes[s] = static_cast<long>(a->batch) * a->hw * cs * 4;
-  }
-  if (nsrc == 1) st->c4[1] = st->c4[0], st->pix[1] = st->pix[0];
-  // consumer threads: the candidate with the fewest idle lanes (a thread owns one channel quad of its source)
-  int best_t = 0;
-  double best_idle = 2.0;
-  for (int t : {256, 320, 384, 448, 512}) {
-    double idle = 0.0;
-    bool ok = true;
-    for (int s = 0; s < nsrc; ++s) {
-      if (st->c4[s] > t) ok = false;
-      else idle += static_cast<double>(bytes[s]) / (bytes[0] + bytes[1]) * (t % st->c4[s]) / t;
-    }
-    if (ok && idle < best_idle - 1e-9) best_idle = idle, best_t = t;
-  }
-  if (best_t == 0) return false;
-  st->consumers = best_t;
-  // 2 CTAs per SM in ONE wave, split between the sources in proportion to their bytes; never more CTAs than stages
-  const int slots = 2 * num_sms();
-  for (int s = 0; s < nsrc; ++s) {
-    long n = nsrc == 1 ? slots : (slots * bytes[s] + (bytes[0] + bytes[1]) / 2) / (bytes[0] + bytes[1]);
-    const long stages = static_cast<long>(a->batch) * (a->hw / st->pix[s]);
-    if (n < 1) n = 1;
-    if (n > stages) n = stages;
-    st->ctas[s] = static_cast<int>(n);
-  }
-  if (nsrc == 1) st->ctas[1] = 0;
-  return true;
-}
-
 extern "C" int ddpo_groupnorm_fwd(const ddpo_groupnorm_args* a, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   GnArgs g;
@@ -798,19 +648,7 @@ extern "C" int ddpo_groupnorm_fwd(const ddpo_groupnorm_args* a, void* stream_) {
     DDPO_LAUNCH_OK();
   }
   if (g.y_bf16 || g.y_f32 || g.raw_bf16) {
-    GnStream st;
-    if (gn_stream_plan(g, a, &st)) {
-      static bool attr = false;
-      const int dyn = GNA_STAGES * GNA_STAGE_BYTES + 128;
-      if (!attr) {
-        DDPO_CUDA_OK(cudaFuncSetAttribute(gn_apply_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn));
-        attr = true;
-      }
-      dim3 sg(st.ctas[0] > st.ctas[1] ? st.ctas[0] : st.ctas[1], 1, a->c1 > 0 ? 2 : 1);
-      gn_apply_tma_kernel<<<sg, 32 + st.consumers, dyn, stream>>>(g, st, a->batch);
-    } else {
-      gn_apply_kernel<<<grid, GN_THREADS, 0, stream>>>(g);
-    }
+    gn_apply_kernel<<<grid, GN_THREADS, 0, stream>>>(g);
     DDPO_LAUNCH_OK();
   }
   return DDPO_OK;
@@ -838,33 +676,16 @@ extern "C" int ddpo_groupnorm_bwd(const ddpo_groupnorm_args* a, const void* dy, 
   }
   DDPO_REQUIRE(smem <= 96 * 1024, "groupnorm_bwd: too many channels (%d)", C);
   DDPO_REQUIRE(b.ldd0 % 4 == 0 && b.ldd1 % 4 == 0, "groupnorm_bwd: gradient pitches must be multiples of 4");
-  // optional ($DDPO_GN_BWD_GROUP_MB > 0): the two passes run over groups of samples whose (x, dy) fit that many MB, so that
-  // pass 2 re-reads from L2 what pass 1 just streamed; a group must still fill the GPU (>= 256 CTAs)
-  const char* gmb = getenv("DDPO_GN_BWD_GROUP_MB");
-  const double group_mb = gmb != nullptr ? atof(gmb) : 0.0;
-  int group = a->batch;
-  if (group_mb > 0.0) {
-    const double bytes_per_sample = static_cast<double>(a->hw) * C * 8.0;
-    group = static_cast<int>(group_mb * 1024 * 1024 / bytes_per_sample);
-    const int min_group = (256 + b.f.chunks - 1) / b.f.chunks;
-    if (group < min_group) group = min_group;
-    if (group > a->batch) group = a->batch;
-  }
-  for (int b0 = 0; b0 < a->batch; b0 += group) {
-    const int nb = a->batch - b0 < group ? a->batch - b0 : group;
-    b.b0 = b0;
-    dim3 g2(b.f.chunks, nb);
-    if (b.dy_bf16) {
-      gn_bwd_stats_kernel<true><<<g2, GN_THREADS, smem, stream>>>(b);
-      DDPO_LAUNCH_OK();
-      gn_bwd_apply_kernel<true><<<g2, GN_THREADS, 0, stream>>>(b);
-    } else {
-      gn_bwd_stats_kernel<false><<<g2, GN_THREADS, smem, stream>>>(b);
-      DDPO_LAUNCH_OK();
-      gn_bwd_apply_kernel<false><<<g2, GN_THREADS, 0, stream>>>(b);
-    }
+  if (b.dy_bf16) {
+    gn_bwd_stats_kernel<true><<<grid, GN_THREADS, smem, stream>>>(b);
     DDPO_LAUNCH_OK();
+    gn_bwd_apply_kernel<true><<<grid, GN_THREADS, 0, stream>>>(b);
+  } else {
+    gn_bwd_stats_kernel<false><<<grid, GN_THREADS, smem, stream>>>(b);
+    DDPO_LAUNCH_OK();
+    gn_bwd_apply_kernel<false><<<grid, GN_THREADS, 0, stream>>>(b);
   }
+  DDPO_LAUNCH_OK();
   launch_reduce_rows(b.dparam_part, 1, a->batch * b.f.chunks, 2 * C, C, dscale, dbias, 1, stream);
   DDPO_LAUNCH_OK();
   return DDPO_OK;

@@ -152,7 +152,7 @@ def ppo_loss(logp, old_logp, adv, clip_range, info_out, dlogp_out, micro_batch=N
 # ------------------------------------------------------------------ GEMM --------
 def igemm(*, a0, wt, n, a1=None, c0=None, c1=0, lda0=None, lda1=None, conv=None, m=None, taps=1, stride=1,
           bias=None, rowvec=None, rows_per_sample=0, rowvec_ld=0, residual=None, ld_res=0, out_f32=None,
-          out_bf16=None, ld_out=0, geglu=False, accumulate=False, bn=0, aux_bf16=None, mt=0, pair=0, epi=0, gn_stats=None,
+          out_bf16=None, ld_out=0, geglu=False, accumulate=False, bn=0, aux_bf16=None, gn_stats=None,
           no_low_pad=False):
     """conv=(batch, h_out, w_out) for convolutions, else linear with m rows."""
     a = IGemmArgs()
@@ -174,9 +174,6 @@ def igemm(*, a0, wt, n, a1=None, c0=None, c1=0, lda0=None, lda1=None, conv=None,
     a.out_f32, a.out_bf16, a.ld_out = _p(out_f32), _p(out_bf16), int(ld_out)
     a.geglu, a.accumulate_out, a.bn_override = int(geglu), int(accumulate), int(bn)
     a.aux_bf16 = _p(aux_bf16)
-    a.mt_override = int(mt)
-    a.pair_override = int(pair)
-    a.epi_override = int(epi)
     a.gn_stats = _p(gn_stats)
     a.conv_pad = int(no_low_pad)
     rows = a.batch * a.h * a.w if a.is_conv else a.m
@@ -324,7 +321,7 @@ def attention_fwd(q, k, v, out, batch, heads, nq, nk, ldq, ldk, ldv, ldo, lse=No
 _WGRAD_WS = {}
 
 
-def wgrad(*, dy, n, x0, dw, x1=None, c0=None, c1=0, ldy=0, ldx0=0, ldx1=0, conv=None, m=None, taps=1, stride=1, kernel=0):
+def wgrad(*, dy, n, x0, dw, x1=None, c0=None, c1=0, ldy=0, ldx0=0, ldx1=0, conv=None, m=None, taps=1, stride=1):
     """dw[(tap, cin), n] += X^T dY (fp32, Flax layout).  conv=(batch, h_out, w_out) or linear with m rows."""
     from ._lib import WgradArgs
     a = WgradArgs()
@@ -338,7 +335,6 @@ def wgrad(*, dy, n, x0, dw, x1=None, c0=None, c1=0, ldy=0, ldx0=0, ldx1=0, conv=
         a.is_conv, a.batch, a.h, a.w, a.m = 0, 0, 0, 0, int(m)
     a.conv_stride, a.taps = int(stride), int(taps)
     a.dw = _p(dw)
-    a.kernel_override = int(kernel)
     need = int(lib().ddpo_wgrad_workspace_floats(C.byref(a)))
     dev = dw.device
     ws = _WGRAD_WS.get(dev)
@@ -358,7 +354,7 @@ def attention_bwd(q, k, v, out, dout, lse, delta, dq, dk, dv, batch, heads, nq, 
                   lddk, lddv):
     from ._lib import AttentionBwdArgs
     a = AttentionBwdArgs(_p(q), _p(k), _p(v), _p(out), _p(dout), _p(lse), _p(delta), _p(dq), _p(dk), _p(dv), batch,
-                         heads, nq, nk, 64, ldq, ldk, ldv, ldo, lddo, lddq, lddk, lddv, None)
+                         heads, nq, nk, 64, ldq, ldk, ldv, ldo, lddo, lddq, lddk, lddv)
     _e = _ev()
     _run("attention_bwd", lib().ddpo_attention_bwd(C.byref(a), _stream()), 14.0 * batch * heads * nq * nk * 64, _e,
          f"B{batch} H{heads} nq{nq} nk{nk}")

@@ -17,7 +17,6 @@ Data flow design:
   * buffers come from a deterministic free-list arena so a whole step can be captured in a
     CUDA graph.
 """
-import os
 from typing import Dict, List, Optional
 
 import numpy as np
@@ -100,8 +99,6 @@ class UNet:
         self.train_mode = False
         # all ResNet time-embedding projections of a pass in ONE launch (ops.dense_small_grouped): bit-identical to the 22
         # separate dense_small launches (tests/test_gpu_kernels.py), each of which runs only 10-40 CTAs.
-        # DDPO_GROUPED_TEMB=0 restores the separate launches.
-        self.grouped_temb = os.environ.get("DDPO_GROUPED_TEMB", "1") == "1"
         self._temb_names = [n[: -len("/time_emb_proj/kernel")] for n in self.table if n.endswith("/time_emb_proj/kernel")]
         self._temb_tables: Dict[int, tuple] = {}
         self._tproj_views: Optional[Dict[str, torch.Tensor]] = None
@@ -224,7 +221,7 @@ class UNet:
         return kv
 
     # ------------------------------------------------------------------ blocks ----
-    def _resnet(self, name, x0, x1, c0, c1, cout, b, h, w, temb_act, tape):
+    def _resnet(self, name, x0, x1, c0, c1, cout, b, h, w, tape):
         A = self.arena
         hw, m, cin = h * w, b * h * w, c0 + c1
         has_sc = (name + "/conv_shortcut/kernel") in self.table
@@ -234,12 +231,7 @@ class UNet:
         raw = A.alloc((m, cin), BF16) if has_sc else None
         ops.groupnorm_fwd(x0, self.p(name + "/norm1/scale"), self.p(name + "/norm1/bias"), gws, b, hw, c0, x1=x1,
                           c1=c1, silu=True, y_bf16=a, raw_bf16=raw, stats0=_st(x0), stats1=_st(x1))
-        if self._tproj_views is not None:
-            tproj = self._tproj_views[name]          # computed by the grouped launch at the start of forward()
-        else:
-            tproj = A.alloc((b, cout), F32)
-            ops.dense_small(temb_act, self.p(name + "/time_emb_proj/kernel"), self.p(name + "/time_emb_proj/bias"),
-                            tproj, b, temb_act.shape[1], cout)
+        tproj = self._tproj_views[name]          # computed by the grouped launch at the start of forward()
         hbuf = A.alloc_with_gn_stats((m, cout), hw)
         ops.igemm(a0=a, wt=self.w[name + "/conv1"], n=cout, c0=cin, conv=(b, h, w), taps=9,
                   bias=self.p(name + "/conv1/bias"), rowvec=tproj, rows_per_sample=hw, rowvec_ld=cout, out_f32=hbuf,
@@ -354,25 +346,22 @@ class UNet:
         temb_act = A.alloc((b, te), F32)
         ops.dense_small(t1, self.p("time_embedding/linear_2/kernel"), self.p("time_embedding/linear_2/bias"), temb_act,
                         b, te, te, silu_out=True)
-        tproj_all = None
-        self._tproj_views = None
-        if self.grouped_temb:
-            tab = self._temb_tables.get(b)
-            if tab is None:   # first (eager, pre-capture) pass at this batch size: offsets only, no addresses
-                entries, views, y_off = [], [], 0
-                for name in self._temb_names:
-                    w_off, wshape = self.table[name + "/time_emb_proj/kernel"]
-                    b_off, _ = self.table[name + "/time_emb_proj/bias"]
-                    n = int(wshape[1])
-                    entries.append((w_off, b_off, y_off, n))
-                    views.append((name, y_off, n))
-                    y_off += b * n
-                dev_tab, ctas = ops.dense_small_group_table(entries, self.device)
-                tab = self._temb_tables[b] = (dev_tab, ctas, views, y_off)
-            dev_tab, ctas, views, total = tab
-            tproj_all = A.alloc((total,), F32)
-            ops.dense_small_grouped(temb_act, self.params, tproj_all, dev_tab, len(views), ctas, b, te)
-            self._tproj_views = {name: tproj_all[o:o + b * n].view(b, n) for name, o, n in views}
+        tab = self._temb_tables.get(b)
+        if tab is None:   # first (eager, pre-capture) pass at this batch size: offsets only, no addresses
+            entries, views, y_off = [], [], 0
+            for name in self._temb_names:
+                w_off, wshape = self.table[name + "/time_emb_proj/kernel"]
+                b_off, _ = self.table[name + "/time_emb_proj/bias"]
+                n = int(wshape[1])
+                entries.append((w_off, b_off, y_off, n))
+                views.append((name, y_off, n))
+                y_off += b * n
+            dev_tab, ctas = ops.dense_small_group_table(entries, self.device)
+            tab = self._temb_tables[b] = (dev_tab, ctas, views, y_off)
+        dev_tab, ctas, views, total = tab
+        tproj_all = A.alloc((total,), F32)
+        ops.dense_small_grouped(temb_act, self.params, tproj_all, dev_tab, len(views), ctas, b, te)
+        self._tproj_views = {name: tproj_all[o:o + b * n].view(b, n) for name, o, n in views}
         x = A.alloc_with_gn_stats((b * H * W, boc[0]), H * W)
         ops.conv_in(latents, self.p("conv_in/kernel"), self.p("conv_in/bias"), x, b, cin_lat, H, W, boc[0], gn_stats=_st(x))
         tap("conv_in", x, (b, H, W, boc[0]))
@@ -385,7 +374,7 @@ class UNet:
         for i, c in enumerate(boc):
             for l in range(cfg.layers_per_block):
                 name = f"down_blocks_{i}/resnets_{l}"
-                y = self._resnet(name, x, None, c_prev, 0, c, b, h, w, temb_act, tape)
+                y = self._resnet(name, x, None, c_prev, 0, c, b, h, w, tape)
                 tap(name, y, (b, h, w, c))
                 x, c_prev = y, c
                 if cfg.down_has_attn[i]:
@@ -412,7 +401,7 @@ class UNet:
                 tap(name, x, (b, h, w, c))
                 skips.append((x, c, h, w))
         cm = boc[-1]
-        y = self._resnet("mid_block/resnets_0", x, None, cm, 0, cm, b, h, w, temb_act, tape)
+        y = self._resnet("mid_block/resnets_0", x, None, cm, 0, cm, b, h, w, tape)
         tap("mid_block/resnets_0", y, (b, h, w, cm))
         x = y
         y = self._transformer("mid_block/attentions_0", x, cm, cfg.attention_head_dim[-1], b, h, w, tape)
@@ -420,7 +409,7 @@ class UNet:
         if tape is None:
             A.release(x)
         x = y
-        y = self._resnet("mid_block/resnets_1", x, None, cm, 0, cm, b, h, w, temb_act, tape)
+        y = self._resnet("mid_block/resnets_1", x, None, cm, 0, cm, b, h, w, tape)
         tap("mid_block/resnets_1", y, (b, h, w, cm))
         if tape is None:
             A.release(x)
@@ -434,7 +423,7 @@ class UNet:
                 sk, sc_, sh, sw = skips.pop()
                 assert (sh, sw) == (h, w)
                 name = f"up_blocks_{i}/resnets_{l}"
-                y = self._resnet(name, x, sk, c_prev, sc_, c, b, h, w, temb_act, tape)
+                y = self._resnet(name, x, sk, c_prev, sc_, c, b, h, w, tape)
                 tap(name, y, (b, h, w, c))
                 if tape is None:
                     A.release(x)
@@ -587,7 +576,7 @@ class UNet:
                                         None, b, c0, te, silu_out=True)
                     for t in (dpre, d_t1, d_temb):
                         A.release(t)
-                for t in (r["sincos"], r["t1"], r["temb_act"], r.get("tproj_all")):
+                for t in (r["sincos"], r["t1"], r["temb_act"], r["tproj_all"]):
                     A.release(t)
         assert not grads, f"{len(grads)} stream gradients were never consumed"
 

@@ -117,11 +117,8 @@ typedef struct {
   int ld_out;
   int geglu;                /* out_bf16[M, n/2] = lin * gelu_tanh(gate); weight rows tile-interleaved */
   int accumulate_out;       /* out_f32 += */
-  int bn_override;          /* 0 = auto; else the tile width: 32, 64, 96, 128, 160, 192, 256 (320 = two 160 tiles) */
+  int bn_override;          /* 0 = auto; else the tile width: 32, 64, 96, 128, 160, 192, 256 */
   void* aux_bf16;           /* GEGLU only, optional: bf16 [M, n] pre-activation (tile-interleaved, bias included) */
-  int mt_override;          /* scheduling hints kept for ABI compatibility; the sm_90a kernel has one tiling and one */
-  int pair_override;        /* epilogue, so these three are accepted and ignored (results never depend on them) */
-  int epi_override;
   int conv_pad;             /* 0 = the 3x3 default (symmetric pad 1); 1 = NO low-side padding: out[y,x] = sum in[s y + dy, s x + dx],
                                reads past the high edge are zero -- the VAE encoder's down-sample (pad ((0,1),(0,1)) + VALID) */
   float* gn_stats;          /* optional, with out_f32: fp32 [ceil(M/32), n, 2] = per 32-row slab and output column the (sum, sum
@@ -225,7 +222,6 @@ typedef struct {
   float* dw;       /* fp32 [taps*(c0+c1), n], accumulated */
   float* workspace;
   int64_t workspace_floats;
-  int kernel_override; /* kept for ABI compatibility; ignored (one weight-gradient kernel) */
 } ddpo_wgrad_args;
 int64_t ddpo_wgrad_workspace_floats(const ddpo_wgrad_args* a);
 int ddpo_wgrad(const ddpo_wgrad_args* a, void* stream);
@@ -238,7 +234,6 @@ typedef struct {
   void* dq; void* dk; void* dv; /* bf16 outputs */
   int batch, heads, nq, nk, head_dim;
   int ldq, ldk, ldv, ldo, lddo, lddq, lddk, lddv;
-  void* workspace;   /* unused, reserved */
 } ddpo_attention_bwd_args;
 int ddpo_attention_bwd(const ddpo_attention_bwd_args* a, void* stream);
 

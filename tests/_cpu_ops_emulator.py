@@ -72,40 +72,6 @@ def groupnorm_fwd(x0, scale, bias, ws, batch, hw, c0, x1=None, c1=0, silu=True, 
         raw_bf16.copy_(x0.reshape(batch * hw, c0).to(BF16))
 
 
-def igemm(*, a0, wt, n, a1=None, c0=None, c1=0, lda0=None, lda1=None, conv=None, m=None, taps=1, stride=1, bias=None,
-          rowvec=None, rows_per_sample=0, rowvec_ld=0, residual=None, ld_res=0, out_f32=None, out_bf16=None, ld_out=0,
-          geglu=False, accumulate=False, bn=0, aux_bf16=None, mt=0, pair=0, epi=0, gn_stats=None, no_low_pad=False):
-    assert a1 is None and not geglu and rowvec is None
-    assert a0.dtype == BF16 and wt.dtype == BF16
-    c0 = int(c0 if c0 is not None else a0.shape[-1])
-    assert c0 % 64 == 0 and n % 32 == 0, (c0, n)
-    w = wt.reshape(n, taps * c0).float()
-    if conv is not None:
-        b, h, wd = conv
-        assert wd & (wd - 1) == 0 and h & (h - 1) == 0
-        x = a0.reshape(b, h * stride, wd * stride, c0).float().permute(0, 3, 1, 2)
-        ks = 3 if taps == 9 else 1
-        wk = w.reshape(n, ks, ks, c0).permute(0, 3, 1, 2)
-        if no_low_pad:      # pad on the high side only, then VALID (the VAE encoder's down-sample)
-            y = F.conv2d(F.pad(x, (0, 1, 0, 1)), wk, None, stride=stride)
-        else:
-            y = F.conv2d(x, wk, None, stride=stride, padding=ks // 2)
-        y = y.permute(0, 2, 3, 1).reshape(b * h * wd, n)
-    else:
-        assert taps == 1
-        y = a0.reshape(m, c0).float() @ w.t()
-    if bias is not None:
-        y = y + bias.reshape(1, n)
-    if residual is not None:
-        y = y + residual.reshape(y.shape)
-    if out_f32 is not None:
-        out_f32.reshape(y.shape).copy_(y)
-    if out_bf16 is not None:
-        out_bf16.reshape(y.shape).copy_(y.to(BF16))
-    if gn_stats is not None:
-        _fill_gn_stats(gn_stats, y)
-
-
 def conv_in(x_nchw, w, bias, y_nhwc, batch, cin, h, wd, cout, gn_stats=None):
     assert cin <= 8 and cout % 4 == 0
     y = F.conv2d(x_nchw, w.permute(3, 2, 0, 1), bias, padding=1).permute(0, 2, 3, 1)
@@ -210,11 +176,6 @@ def gather_rows(src, index, dst):
     dst.copy_(src.reshape(-1, dst.shape[-1])[index.long()].reshape(dst.shape))
 
 
-def dense_small(x, w, bias, y, batch, k, n, silu_in=False, silu_out=False):
-    assert not silu_in and not silu_out
-    y.copy_(x.reshape(batch, k) @ w.reshape(k, n) + bias)
-
-
 # ---- U-Net forward (sampling path) ----
 import math  # noqa: E402
 
@@ -258,7 +219,7 @@ def timestep_sincos(t, out, batch, dim):
 _silu = lambda v: v * torch.sigmoid(v)
 
 
-def dense_small(x, w, bias, y, batch, k, n, silu_in=False, silu_out=False):  # noqa: F811
+def dense_small(x, w, bias, y, batch, k, n, silu_in=False, silu_out=False):
     xv = x.reshape(batch, k)
     r = (_silu(xv) if silu_in else xv) @ w.reshape(k, n) + (bias if bias is not None else 0)
     y.copy_(_silu(r) if silu_out else r)
@@ -293,10 +254,12 @@ def groupnorm_fwd(x0, scale, bias, ws, batch, hw, c0, x1=None, c1=0, silu=True, 
                              st)
 
 
-def igemm(*, a0, wt, n, a1=None, c0=None, c1=0, lda0=None, lda1=None, conv=None, m=None, taps=1, stride=1, bias=None,  # noqa: F811
+def igemm(*, a0, wt, n, a1=None, c0=None, c1=0, lda0=None, lda1=None, conv=None, m=None, taps=1, stride=1, bias=None,
           rowvec=None, rows_per_sample=0, rowvec_ld=0, residual=None, ld_res=0, out_f32=None, out_bf16=None, ld_out=0,
-          geglu=False, accumulate=False, bn=0, aux_bf16=None, mt=0, pair=0, epi=0, gn_stats=None, no_low_pad=False):
+          geglu=False, accumulate=False, bn=0, aux_bf16=None, gn_stats=None, no_low_pad=False):
     assert a0.dtype == BF16 and wt.dtype == BF16 and (a1 is None or a1.dtype == BF16)
+    if conv is None and a0.dim() == 2 and c0 is not None and a0.shape[1] != c0:
+        a0 = a0[:, :c0].contiguous()     # a column-offset view of a wider matrix as the linear A operand (lda0 = its pitch)
     c0 = int(c0 if c0 is not None else a0.shape[-1])
     cin = c0 + c1
     assert c0 % 64 == 0 and c1 % 64 == 0 and n % 32 == 0, (c0, c1, n)
@@ -388,7 +351,7 @@ def _patches(x_nhwc, taps, stride):
     return u
 
 
-def wgrad(*, dy, n, x0, dw, x1=None, c0=None, c1=0, ldy=0, ldx0=0, ldx1=0, conv=None, m=None, taps=1, stride=1, kernel=0):
+def wgrad(*, dy, n, x0, dw, x1=None, c0=None, c1=0, ldy=0, ldx0=0, ldx1=0, conv=None, m=None, taps=1, stride=1):
     c0 = int(c0 if c0 is not None else x0.shape[-1])
     if conv is not None:
         b, h, wd = conv
@@ -504,16 +467,6 @@ def dense_small_bwd(x, w, bias, dy, dpre_ws, dw, db, dx, batch, k, n, silu_in=Fa
     db.add_(bz.grad)
     if dx is not None:
         dx.reshape(batch, k).copy_(dx.reshape(batch, k) + xv.grad if dx_accumulate else xv.grad)
-
-
-_igemm_fwd = igemm
-
-
-def igemm(*, a0, lda0=None, c0=None, m=None, conv=None, **kw):  # noqa: F811
-    """column-offset views of wider matrices as the linear A operand (lda0 = pitch of the parent)"""
-    if conv is None and a0.dim() == 2 and c0 is not None and a0.shape[1] != c0:
-        a0 = a0[:, :c0].contiguous()
-    return _igemm_fwd(a0=a0, lda0=lda0, c0=c0, m=m, conv=conv, **kw)
 
 
 # ---- scheduler / PPO / optimizer ops (sampler + train_step dry runs); host-only helpers come from the real module ----

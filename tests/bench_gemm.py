@@ -1,4 +1,4 @@
-"""Micro-benchmark (not a test): igemm variants on a few representative shapes. Usage: python tests/bench_gemm.py"""
+"""Micro-benchmark (not a test): igemm with fp32 and bf16 outputs on a few representative shapes. Usage: python tests/bench_gemm.py"""
 import math, os, sys, time
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -31,17 +31,16 @@ def run(name, m=None, k=None, n=None, conv=None, c=None, taps=9, bn=0, res=False
     outb = torch.zeros(m, n, dtype=torch.bfloat16, device=dev)
     r = torch.randn(m, n, device=dev) if res else None
     line = [name]
-    for label, kw in (("1cta", dict(pair=2, mt=1)), ("fat", dict(pair=2, mt=2)), ("pair", dict(pair=1))):
-        for outk in ("f32", "bf16"):
-            def fn():
-                if conv is None:
-                    ops.igemm(a0=a, wt=w, n=n, c0=k, m=m, residual=r, out_f32=out if outk == "f32" else None,
-                              out_bf16=outb if outk == "bf16" else None, bn=bn, **kw)
-                else:
-                    ops.igemm(a0=a, wt=w, n=n, c0=c, conv=(conv[0], conv[1], conv[1]), taps=taps, residual=r,
-                              out_f32=out if outk == "f32" else None, out_bf16=outb if outk == "bf16" else None, bn=bn, **kw)
-            t = timeit(fn)
-            line.append(f"{label}/{outk}: {flops / t / 1e12:7.1f} TF/s ({t * 1e6:7.1f} us)")
+    for outk in ("f32", "bf16"):
+        def fn():
+            if conv is None:
+                ops.igemm(a0=a, wt=w, n=n, c0=k, m=m, residual=r, out_f32=out if outk == "f32" else None,
+                          out_bf16=outb if outk == "bf16" else None, bn=bn)
+            else:
+                ops.igemm(a0=a, wt=w, n=n, c0=c, conv=(conv[0], conv[1], conv[1]), taps=taps, residual=r,
+                          out_f32=out if outk == "f32" else None, out_bf16=outb if outk == "bf16" else None, bn=bn)
+        t = timeit(fn)
+        line.append(f"{outk}: {flops / t / 1e12:7.1f} TF/s ({t * 1e6:7.1f} us)")
     print(" | ".join(line), flush=True)
 
 run("linear 16384x1280x8192 bn256", m=16384, k=8192, n=1280)

@@ -1,4 +1,4 @@
-"""Micro-benchmark (not a test): low-resolution convolutions (few CTA tiles) across BN / kernel choices."""
+"""Micro-benchmark (not a test): low-resolution convolutions (few CTA tiles) across tile widths BN."""
 import os, sys, math
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -21,7 +21,6 @@ for (b, h, c, n) in [(40, 8, 1280, 1280), (16, 8, 1280, 1280), (40, 16, 1280, 12
     out = torch.zeros(b * h * h, n, device=dev)
     line = [f"conv {b}x{h}x{h} c{c}->{n}"]
     for bn in (0, 256, 160, 128, 64):
-        for pair in (1, 2):
-            t = timeit(lambda: ops.igemm(a0=a, wt=w, n=n, c0=c, conv=(b, h, h), taps=9, out_f32=out, bn=bn, pair=pair))
-            line.append(f"bn{bn}/{'pair' if pair == 1 else '1cta'} {t:6.1f}us")
+        t = timeit(lambda: ops.igemm(a0=a, wt=w, n=n, c0=c, conv=(b, h, h), taps=9, out_f32=out, bn=bn))
+        line.append(f"bn{bn} {t:6.1f}us")
     print(" | ".join(line), flush=True)

@@ -1,4 +1,4 @@
-"""ncu / timing target (not a test): GroupNorm forward (finalize + streamed apply), GroupNorm backward and LayerNorm at the
+"""ncu / timing target (not a test): GroupNorm forward (finalize + apply), GroupNorm backward and LayerNorm at the
 U-Net's dominant shapes.
     python tests/prof_norm.py                       # CUDA-event timings -> achieved GB/s on ALGORITHMIC bytes
     ncu --set full --clock-control none --import-source on -k regex:"gn_|layernorm" -c 24 -o gpurun_out/r2_norm_full \
@@ -116,11 +116,6 @@ def ln_bwd(m, c):
 
 gn_fwd(16, 4096, 320, 0)            # the dominant sampling shape
 gn_fwd(16, 4096, 320, 0, with_stats=False, tag="[two-pass]")
-if not once:
-    os.environ["DDPO_GN_STREAM"] = "1"
-    gn_fwd(16, 4096, 320, 0, tag="[TMA-streamed apply]")
-    gn_fwd(40, 4096, 320, 0, tag="[TMA-streamed apply]")
-    os.environ["DDPO_GN_STREAM"] = "0"
 gn_fwd(16, 4096, 640, 320)          # up_blocks_3 concat
 gn_fwd(16, 1024, 640, 0)
 gn_fwd(16, 256, 1280, 1280)
@@ -129,12 +124,8 @@ ln_fwd(65536, 320)
 ln_fwd(16384, 640)
 ln_fwd(4096, 1280)
 if not once:
-    for mb in ("0", "64", "96"):
-        os.environ["DDPO_GN_BWD_GROUP_MB"] = mb
-        print(f"DDPO_GN_BWD_GROUP_MB={mb}")
-        gn_bwd(40, 4096, 320)
-        gn_bwd(40, 1024, 640)
-    os.environ["DDPO_GN_BWD_GROUP_MB"] = "0"
+    gn_bwd(40, 4096, 320)
+    gn_bwd(40, 1024, 640)
     ln_bwd(163840, 320)
     ln_bwd(40960, 640)
 print("done")

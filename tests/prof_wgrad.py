@@ -28,9 +28,8 @@ def t(fn, n=10):
     return e0.elapsed_time(e1) / n * 1e3
 
 
-for kern in (0, 2):
-    a = t(lambda: ops.wgrad(dy=dy, n=320, x0=x, c0=320, conv=(B, 64, 64), taps=9, dw=dw9, kernel=kern))
-    b = t(lambda: ops.wgrad(dy=dy, n=320, x0=x, c0=320, m=B * 4096, dw=dw1, kernel=kern))
-    c = t(lambda: ops.wgrad(dy=dy2, n=1280, x0=x2, c0=1280, conv=(B, 16, 16), taps=9, dw=dw2, kernel=kern))
-    print(f"kernel {kern}: conv3x3 320->320 {a:.1f} us ({2 * B * 4096 * 2880 * 320 / a / 1e6:.0f} TF/s) | linear 320x320 {b:.1f} us | "
-          f"conv3x3 1280->1280 @16x16 {c:.1f} us ({2 * B * 256 * 11520 * 1280 / c / 1e6:.0f} TF/s)")
+a = t(lambda: ops.wgrad(dy=dy, n=320, x0=x, c0=320, conv=(B, 64, 64), taps=9, dw=dw9))
+b = t(lambda: ops.wgrad(dy=dy, n=320, x0=x, c0=320, m=B * 4096, dw=dw1))
+c = t(lambda: ops.wgrad(dy=dy2, n=1280, x0=x2, c0=1280, conv=(B, 16, 16), taps=9, dw=dw2))
+print(f"conv3x3 320->320 {a:.1f} us ({2 * B * 4096 * 2880 * 320 / a / 1e6:.0f} TF/s) | linear 320x320 {b:.1f} us | "
+      f"conv3x3 1280->1280 @16x16 {c:.1f} us ({2 * B * 256 * 11520 * 1280 / c / 1e6:.0f} TF/s)")

@@ -26,7 +26,7 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(L, f), f"{f} declared in include/ddpo_b200.h but not exported"
     assert sorted(_lib.SIGNATURES) == fns, set(fns) ^ set(_lib.SIGNATURES)
     lib = _lib.lib()
-    assert lib.ddpo_abi_version() == 2
+    assert lib.ddpo_abi_version() == 3
 
 
 def test_no_gpu_calls_fail_loudly():

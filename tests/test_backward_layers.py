@@ -592,15 +592,3 @@ def test_groupnorm_bwd_resnet_norm1(b, h, w, c0, c1):
     check_sum("dscale", dsc, scr.grad, (dyp * xhat).abs().sum(dim=(0, 2)), tol=2 * SUM_TOL, old=case["dsc_old"].to(dev))
     check_sum("dbias", dbi, bir.grad, dyp.abs().sum(dim=(0, 2)), tol=2 * SUM_TOL, old=case["dbi_old"].to(dev))
 
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("b,h,w,c0,c1", [(40, 64, 64, 320, 0), (40, 32, 32, 640, 320)])
-def test_groupnorm_bwd_sample_groups_bit_identical(monkeypatch, b, h, w, c0, c1):
-    """$DDPO_GN_BWD_GROUP_MB runs the two passes over groups of samples (here 5 launches of 8 samples): same bits"""
-    hw = h * w
-    case = _gn_case(b, h, w, c0, c1, 67)
-    monkeypatch.delenv("DDPO_GN_BWD_GROUP_MB", raising=False)
-    ref = _gn_run(case, b, hw, c0, c1)
-    monkeypatch.setenv("DDPO_GN_BWD_GROUP_MB", "32")
-    got = _gn_run(case, b, hw, c0, c1)
-    assert all(torch.equal(x, y) for x, y in zip(ref, got))

@@ -12,10 +12,9 @@ def bf(x):
     return x.to(torch.bfloat16)
 
 
-@pytest.mark.parametrize("kernel", [0, 2])  # kernel_override: a hint the library ignores
 @pytest.mark.parametrize("m,k,n", [(256, 64, 64), (1000, 320, 320), (4096, 1280, 640), (154, 1024, 1280), (8192, 128, 960),
                                    (5000, 192, 192), (40960, 320, 2560)])
-def test_wgrad_linear(m, k, n, kernel):
+def test_wgrad_linear(m, k, n):
     from ddpo_b200 import ops
     g = torch.Generator(device="cpu").manual_seed(0)
     x = bf(torch.randn(m, k, generator=g)).to(DEV)
@@ -23,7 +22,7 @@ def test_wgrad_linear(m, k, n, kernel):
     dyw = bf(torch.randn(m, n + 64, generator=g)).to(DEV)
     dy = dyw[:, :n]
     dw = torch.ones(k, n, device=DEV)
-    ops.wgrad(dy=dy, ldy=n + 64, n=n, x0=x, c0=k, m=m, dw=dw, kernel=kernel)
+    ops.wgrad(dy=dy, ldy=n + 64, n=n, x0=x, c0=k, m=m, dw=dw)
     torch.cuda.synchronize()
     ref = 1.0 + x.float().t() @ dy.float()
     err = (dw - ref).abs().max().item()
@@ -34,8 +33,7 @@ def test_wgrad_linear(m, k, n, kernel):
                                                    (2, 32, 320, 0, 320, 3, 1), (2, 16, 64, 64, 128, 1, 1),
                                                    (2, 8, 64, 0, 64, 3, 2), (3, 4, 64, 0, 64, 3, 1),
                                                    (2, 16, 320, 640, 320, 3, 1), (1, 8, 192, 0, 448, 3, 1)])
-@pytest.mark.parametrize("kernel", [0, 2])
-def test_wgrad_conv(b, h, c0, c1, n, ks, stride, kernel):
+def test_wgrad_conv(b, h, c0, c1, n, ks, stride):
     from ddpo_b200 import ops
     g = torch.Generator(device="cpu").manual_seed(1)
     hi = h * stride
@@ -44,7 +42,7 @@ def test_wgrad_conv(b, h, c0, c1, n, ks, stride, kernel):
     dy = bf(torch.randn(b * h * h, n, generator=g)).to(DEV)
     cin = c0 + c1
     dw = torch.zeros(ks * ks * cin, n, device=DEV)
-    ops.wgrad(dy=dy, n=n, x0=x0, x1=x1, c0=c0, c1=c1, conv=(b, h, h), taps=ks * ks, stride=stride, dw=dw, kernel=kernel)
+    ops.wgrad(dy=dy, n=n, x0=x0, x1=x1, c0=c0, c1=c1, conv=(b, h, h), taps=ks * ks, stride=stride, dw=dw)
     torch.cuda.synchronize()
     xin = (x0.float() if x1 is None else torch.cat([x0.float(), x1.float()], -1)).permute(0, 3, 1, 2).requires_grad_(False)
     w = torch.zeros(n, cin, ks, ks, device=DEV, requires_grad=True)

@@ -67,10 +67,9 @@ def test_post_quant_and_conv_out():
                                rtol=1e-4, atol=1e-5)
 
 
-@pytest.mark.parametrize("b,h,w,c,n,ks,pair", [(1, 4, 256, 64, 64, 3, 0), (2, 256, 256, 64, 64, 3, 0),
-                                               (1, 8, 512, 64, 128, 3, 0), (1, 4, 256, 128, 64, 1, 0),
-                                               (1, 8, 256, 64, 64, 3, 2), (2, 2, 1024, 64, 64, 3, 0)])
-def test_igemm_conv_rows_wider_than_a_tile(b, h, w, c, n, ks, pair):
+@pytest.mark.parametrize("b,h,w,c,n,ks", [(1, 4, 256, 64, 64, 3), (2, 256, 256, 64, 64, 3), (1, 8, 512, 64, 128, 3),
+                                          (1, 4, 256, 128, 64, 1), (1, 8, 256, 64, 64, 3), (2, 2, 1024, 64, 64, 3)])
+def test_igemm_conv_rows_wider_than_a_tile(b, h, w, c, n, ks):
     """W > 128: a pixel row spans W/128 tiles; left/right zero padding must come from the TMA box at x = -1 / W"""
     from ddpo_b200 import ops
     g = torch.Generator().manual_seed(2)
@@ -80,7 +79,7 @@ def test_igemm_conv_rows_wider_than_a_tile(b, h, w, c, n, ks, pair):
     res = torch.randn(b * h * w, n, generator=g).to(DEV)
     out = torch.zeros(b * h * w, n, device=DEV)
     ops.igemm(a0=x, wt=_prep_w(wk.reshape(ks * ks * c, n)), n=n, c0=c, conv=(b, h, w), taps=ks * ks, bias=bias,
-              residual=res, out_f32=out, pair=pair)
+              residual=res, out_f32=out)
     torch.cuda.synchronize()
     ref = torch.nn.functional.conv2d(x.float().permute(0, 3, 1, 2), bf(wk).float().permute(3, 2, 0, 1), bias,
                                      padding=ks // 2).permute(0, 2, 3, 1).reshape(b * h * w, n) + res

@@ -1,8 +1,6 @@
-"""The grouped time-embedding projection launch (bit-identical to the separate launches; default ON: one launch instead
-of one per ResNet block) and the aesthetic reward model on the GPU kernels (CLIP ViT image
+"""The grouped time-embedding projection launch (one launch instead of one per ResNet block, bit-identical to the
+separate launches) and the aesthetic reward model on the GPU kernels (CLIP ViT image
 tower + LAION head against the oracle pinned to `transformers`)."""
-import os
-
 import numpy as np
 import pytest
 import torch
@@ -40,8 +38,10 @@ def test_dense_small_grouped_is_bit_identical(batch):
 
 
 @pytest.mark.parametrize("cfg_name,batch", [("TINY", 2), ("SMALL", 4)])
-def test_unet_with_grouped_temb_is_bit_identical(cfg_name, batch, monkeypatch):
-    from ddpo_b200 import unet_spec
+def test_unet_grouped_temb_matches_separate_launches(cfg_name, batch):
+    """Each of the 22 projections the U-Net's grouped launch wrote (at its real parameter-table offsets) equals a separate
+    dense_small launch on that block's own time_emb_proj parameters and the same silu(temb)"""
+    from ddpo_b200 import ops, unet_spec
     from ddpo_b200.unet import UNet
     cfg = getattr(unet_spec, cfg_name)
     flat = unet_spec.init_flat_params(cfg, 0)
@@ -49,20 +49,21 @@ def test_unet_with_grouped_temb_is_bit_identical(cfg_name, batch, monkeypatch):
     lat = torch.randn(batch, 4, cfg.sample_size, cfg.sample_size, generator=g).to(DEV)
     ctx = torch.randn(batch, cfg.ctx_len, cfg.cross_attention_dim, generator=g).to(DEV)
     ts = torch.tensor([981, 441, 21, 1][:batch], dtype=torch.int32, device=DEV)
-    outs = []
-    for flag in ("0", "1"):
-        monkeypatch.setenv("DDPO_GROUPED_TEMB", flag)
-        net = UNet(cfg, flat, DEV)
-        assert net.grouped_temb == (flag == "1")
-        net.prepare_context(ctx)
-        outs.append(net.forward(lat, ts).clone())
-        net.enable_training()      # and through the taped forward + backward
-        tape = []
-        eps = net.forward(lat, ts, tape=tape)
-        net.backward(tape, torch.ones_like(eps) / eps.numel())
-        outs.append(net.grads.clone())
-    torch.cuda.synchronize()
-    assert torch.equal(outs[0], outs[2]) and torch.equal(outs[1], outs[3])
+    net = UNet(cfg, flat, DEV)
+    net.prepare_context(ctx)
+    net.enable_training()
+    tape = []
+    net.forward(lat, ts, tape=tape)    # with a tape the arena keeps temb_act and the grouped output alive
+    temb_act = next(d for kind, d in tape if kind == "head")["temb_act"]
+    te = temb_act.shape[1]
+    assert len(net._tproj_views) == 22
+    for name, got in net._tproj_views.items():
+        w, bias = net.p(name + "/time_emb_proj/kernel"), net.p(name + "/time_emb_proj/bias")
+        n = w.shape[1]
+        ref = torch.empty(batch, n, device=DEV)
+        ops.dense_small(temb_act, w, bias, ref, batch, te, n)
+        torch.cuda.synchronize()
+        assert torch.equal(got, ref), name
 
 
 # ------------------------------------------------------------------ aesthetic reward model (clip_vision.py) ----

@@ -1,7 +1,7 @@
 """The U-Net's HOST assembly (ddpo_b200/unet.py: kernel sequencing of the sampling forward, weight preparation incl. the
 GEGLU tile interleave, two-source norms / convolutions, cross-attention K/V cache, skip bookkeeping) dry-run on the
-torch-CPU emulation of the ops it calls (tests/_cpu_ops_emulator.py) against the oracle -- and the default-off grouped
-time-embedding path against the default one.  The CUDA kernels themselves are checked on the GPU box."""
+torch-CPU emulation of the ops it calls (tests/_cpu_ops_emulator.py) against the oracle -- and the grouped
+time-embedding launch against per-block launches.  The CUDA kernels themselves are checked on the GPU box."""
 import os
 import sys
 
@@ -12,12 +12,11 @@ import torch
 sys.path.insert(0, os.path.dirname(__file__))
 
 
-def _net(monkeypatch, cfg, flat, grouped):
+def _net(monkeypatch, cfg, flat):
     import _cpu_ops_emulator as E
     from ddpo_b200 import unet as U
     monkeypatch.setattr(U, "ops", E)
     monkeypatch.setattr(U, "Arena", E.CpuArena)
-    monkeypatch.setenv("DDPO_GROUPED_TEMB", "1" if grouped else "0")
     return U.UNet(cfg, flat, device="cpu")
 
 
@@ -31,7 +30,7 @@ def test_unet_forward_host_assembly_matches_oracle(monkeypatch, batch, scalar_t)
     lat = torch.randn(batch, 4, cfg.sample_size, cfg.sample_size, generator=g)
     ctx = torch.randn(batch, cfg.ctx_len, cfg.cross_attention_dim, generator=g)
     ts = torch.tensor([981] if scalar_t else [981, 21, 441][:batch], dtype=torch.int32)
-    net = _net(monkeypatch, cfg, flat, grouped=False)
+    net = _net(monkeypatch, cfg, flat)
     net.prepare_context(ctx)
     eps = net.forward(lat, ts)
     with torch.no_grad():
@@ -47,7 +46,10 @@ def test_unet_forward_host_assembly_matches_oracle(monkeypatch, batch, scalar_t)
     assert torch.equal(net.forward(lat, ts), eps)
 
 
-def test_grouped_time_embedding_path_equals_default(monkeypatch):
+def test_grouped_time_embedding_matches_per_block_dense_small(monkeypatch):
+    """each block's projection from the grouped launch (at the U-Net's parameter-table offsets) equals a separate
+    dense_small on that block's own time_emb_proj parameters"""
+    import _cpu_ops_emulator as E
     from ddpo_b200 import unet_spec
     cfg = unet_spec.TINY
     flat = unet_spec.init_flat_params(cfg, 0)
@@ -55,16 +57,20 @@ def test_grouped_time_embedding_path_equals_default(monkeypatch):
     lat = torch.randn(2, 4, cfg.sample_size, cfg.sample_size, generator=g)
     ctx = torch.randn(2, cfg.ctx_len, cfg.cross_attention_dim, generator=g)
     ts = torch.tensor([500, 3], dtype=torch.int32)
-    outs = []
-    for grouped in (False, True):
-        net = _net(monkeypatch, cfg, flat, grouped)
-        assert net.grouped_temb == grouped and len(net._temb_names) == 22
-        net.prepare_context(ctx)
-        outs.append(net.forward(lat, ts))
-        if grouped:
-            tab = net._temb_tables[2]
-            assert tab[1] == sum((n + 31) // 32 for _, _, n in tab[2])       # CTA count of the grouped launch
-    np.testing.assert_allclose(outs[0].numpy(), outs[1].numpy(), rtol=1e-5, atol=1e-6)
+    net = _net(monkeypatch, cfg, flat)
+    net.enable_training()
+    net.prepare_context(ctx)
+    tape = []
+    net.forward(lat, ts, tape=tape)
+    temb_act = next(d for kind, d in tape if kind == "head")["temb_act"]
+    assert len(net._temb_names) == 22 and sorted(net._tproj_views) == sorted(net._temb_names)
+    for name, got in net._tproj_views.items():
+        w, bias = net.p(name + "/time_emb_proj/kernel"), net.p(name + "/time_emb_proj/bias")
+        ref = torch.empty(2, w.shape[1])
+        E.dense_small(temb_act, w, bias, ref, 2, w.shape[0], w.shape[1])
+        assert torch.equal(got, ref), name
+    tab = net._temb_tables[2]
+    assert tab[1] == sum((n + 31) // 32 for _, _, n in tab[2])       # CTA count of the grouped launch
 
 
 @pytest.mark.parametrize("batch", [2])
@@ -82,7 +88,7 @@ def test_unet_backward_host_assembly_matches_oracle_autograd(monkeypatch, batch)
     ctx = torch.randn(batch, cfg.ctx_len, cfg.cross_attention_dim, generator=g)
     ts = torch.tensor([981, 21][:batch], dtype=torch.int32)
     d_eps = torch.randn(batch, 4, s, s, generator=g) / (4 * s * s)
-    net = _net(monkeypatch, cfg, flat, grouped=False)
+    net = _net(monkeypatch, cfg, flat)
     net.enable_training()
     net.prepare_context(ctx)
     tape = []
