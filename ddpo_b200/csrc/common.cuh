@@ -37,6 +37,12 @@ int make_tensor_map(CUtensorMap* out, const void* base, int elem_bytes, int rank
                     const uint64_t* strides_bytes /* rank-1 entries, dims 1.. */, const uint32_t* box,
                     const uint32_t* elem_strides, int swizzle_128b);
 
+// An attention operand or output: bf16 [batch, n, ld] with head h at columns [h d, h d + d).  TMA and the 16-byte loads
+// of the attention kernels need a 16-byte aligned base and a row pitch of whole 16-byte units.
+inline bool attention_operands_ok(const void* base, int ld, int heads, int d) {
+  return (reinterpret_cast<uintptr_t>(base) & 15) == 0 && ld % 8 == 0 && ld >= heads * d;
+}
+
 #ifdef __CUDACC__
 // ------------------------------------------------------------- small utils ----
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {

@@ -310,10 +310,15 @@ def dense_small_grouped(x, params_base, y_base, table, n_groups, total_ctas, bat
 
 
 # --------------------------------------------------------------- attention -------
-def attention_fwd(q, k, v, out, batch, heads, nq, nk, ldq, ldk, ldv, ldo, lse=None, causal=False):
-    a = AttentionArgs(_p(q), _p(k), _p(v), _p(out), _p(lse), batch, heads, nq, nk, 64, ldq, ldk, ldv, ldo, int(causal))
+ATTENTION_HEAD_DIMS = (40, 64, 80, 160)   # what ddpo_attention_fwd / _bwd accept (SD2: 64; SD1.x: 40, 80, 160)
+
+
+def attention_fwd(q, k, v, out, batch, heads, nq, nk, ldq, ldk, ldv, ldo, lse=None, causal=False, head_dim=64):
+    """head h of q/k/v/out at columns [h * head_dim, (h + 1) * head_dim); head_dim is 40, 64, 80 or 160"""
+    a = AttentionArgs(_p(q), _p(k), _p(v), _p(out), _p(lse), batch, heads, nq, nk, head_dim, ldq, ldk, ldv, ldo,
+                      int(causal))
     _e = _ev()
-    _run("attention_fwd", lib().ddpo_attention_fwd(C.byref(a), _stream()), 4.0 * batch * heads * nq * nk * 64, _e,
+    _run("attention_fwd", lib().ddpo_attention_fwd(C.byref(a), _stream()), 4.0 * batch * heads * nq * nk * head_dim, _e,
          f"B{batch} H{heads} nq{nq} nk{nk}")
 
 
@@ -351,12 +356,12 @@ def wgrad(*, dy, n, x0, dw, x1=None, c0=None, c1=0, ldy=0, ldx0=0, ldx1=0, conv=
 
 # ------------------------------------------------------- backward wrappers -------
 def attention_bwd(q, k, v, out, dout, lse, delta, dq, dk, dv, batch, heads, nq, nk, ldq, ldk, ldv, ldo, lddo, lddq,
-                  lddk, lddv):
+                  lddk, lddv, head_dim=64):
     from ._lib import AttentionBwdArgs
     a = AttentionBwdArgs(_p(q), _p(k), _p(v), _p(out), _p(dout), _p(lse), _p(delta), _p(dq), _p(dk), _p(dv), batch,
-                         heads, nq, nk, 64, ldq, ldk, ldv, ldo, lddo, lddq, lddk, lddv)
+                         heads, nq, nk, head_dim, ldq, ldk, ldv, ldo, lddo, lddq, lddk, lddv)
     _e = _ev()
-    _run("attention_bwd", lib().ddpo_attention_bwd(C.byref(a), _stream()), 14.0 * batch * heads * nq * nk * 64, _e,
+    _run("attention_bwd", lib().ddpo_attention_bwd(C.byref(a), _stream()), 14.0 * batch * heads * nq * nk * head_dim, _e,
          f"B{batch} H{heads} nq{nq} nk{nk}")
 
 

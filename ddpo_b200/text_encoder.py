@@ -46,6 +46,9 @@ TEXT_TINY_QUICK = CLIPTextConfig(vocab_size=1000, hidden_size=192, intermediate_
 
 def text_config_for(pretrained_model):
     """the text tower that conditions the U-Net of ``pretrained_model`` (hidden size == cross_attention_dim)"""
+    from .utils.serialization import MODEL_CONFIGS
+    if MODEL_CONFIGS.get(pretrained_model) == "SD1":
+        return SD1_TEXT
     return {"tiny": CLIPTextConfig(vocab_size=49408, hidden_size=64, intermediate_size=256, num_hidden_layers=2,
                                    num_attention_heads=1),
             "small": CLIPTextConfig(vocab_size=49408, hidden_size=128, intermediate_size=512, num_hidden_layers=2,

@@ -23,6 +23,7 @@ import numpy as np
 import torch
 
 from . import ops
+from .ops import ATTENTION_HEAD_DIMS
 from .unet_spec import UNetConfig, param_offsets
 
 BF16 = torch.bfloat16
@@ -76,11 +77,20 @@ class Arena:
             t._ddpo_raw = None
 
 
+def _head_dim_kw(c, heads):
+    """the ``head_dim`` keyword of the ops' attention calls: omitted at 64, the ops' default, so that an ops module without
+    the keyword (the torch-CPU emulation the host-assembly dry runs use, tests/_cpu_ops_emulator.py) runs the SD2 family"""
+    d = c // heads
+    return {} if d == 64 else {"head_dim": d}
+
+
 class UNet:
     def __init__(self, cfg: UNetConfig, flat_params: torch.Tensor, device="cuda"):
         assert all(c % 64 == 0 for c in cfg.block_out_channels), "channel counts must be multiples of 64"
         for c, h in zip(cfg.block_out_channels, cfg.attention_head_dim):
-            assert c // h == 64, "only head_dim 64 (SD2 family) is implemented"
+            assert c % h == 0 and c // h in ATTENTION_HEAD_DIMS, \
+                f"{c} channels over {h} heads: the attention kernels take head dims {ATTENTION_HEAD_DIMS} " \
+                "(SD2: 64, SD1.x: 40, 80, 160)"
         assert cfg.cross_attention_dim % 64 == 0
         self.cfg = cfg
         self.device = torch.device(device)
@@ -277,7 +287,8 @@ class UNet:
         ops.igemm(a0=ln1, wt=self.w[bl + "/attn1/qkv"], n=3 * c, c0=c, m=m, out_bf16=qkv)
         ao1 = A.alloc((m, c), BF16)
         lse1 = A.alloc((b, heads, hw), F32) if tape is not None else None
-        ops.attention_fwd(qkv, qkv[:, c:], qkv[:, 2 * c:], ao1, b, heads, hw, hw, 3 * c, 3 * c, 3 * c, c, lse=lse1)
+        ops.attention_fwd(qkv, qkv[:, c:], qkv[:, 2 * c:], ao1, b, heads, hw, hw, 3 * c, 3 * c, 3 * c, c, lse=lse1,
+                          **_head_dim_kw(c, heads))
         h1 = A.alloc((m, c), F32)
         ops.igemm(a0=ao1, wt=self.w[bl + "/attn1/to_out_0"], n=c, c0=c, m=m, bias=self.p(bl + "/attn1/to_out_0/bias"),
                   residual=h0, out_f32=h1)
@@ -290,7 +301,8 @@ class UNet:
         kv = self.ctx_kv[bl + "/attn2/kv"]
         ao2 = A.alloc((m, c), BF16)
         lse2 = A.alloc((b, heads, hw), F32) if tape is not None else None
-        ops.attention_fwd(q2, kv, kv[:, c:], ao2, b, heads, hw, L, c, 2 * c, 2 * c, c, lse=lse2)
+        ops.attention_fwd(q2, kv, kv[:, c:], ao2, b, heads, hw, L, c, 2 * c, 2 * c, c, lse=lse2,
+                          **_head_dim_kw(c, heads))
         h2 = A.alloc((m, c), F32)
         ops.igemm(a0=ao2, wt=self.w[bl + "/attn2/to_out_0"], n=c, c0=c, m=m, bias=self.p(bl + "/attn2/to_out_0/bias"),
                   residual=h1, out_f32=h2)
@@ -698,7 +710,7 @@ class UNet:
         dkv = A.alloc((b * L, 2 * c), BF16)
         delta = A.alloc((b, heads, hw), F32)
         ops.attention_bwd(t["q2"], kv, kv[:, c:], t["ao2"], d_ao, t["lse2"], delta, dq2, dkv, dkv[:, c:], b, heads, hw, L,
-                          c, 2 * c, 2 * c, c, c, c, 2 * c, 2 * c)
+                          c, 2 * c, 2 * c, c, c, c, 2 * c, 2 * c, **_head_dim_kw(c, heads))
         ops.wgrad(dy=dq2, n=c, x0=t["ln2"], c0=c, m=m, dw=self.g(bl + "/attn2/to_q/kernel"))
         ops.wgrad(dy=dkv, ldy=2 * c, n=c, x0=self._ctx_bf, c0=dctx, m=b * L, dw=self.g(bl + "/attn2/to_k/kernel"))
         ops.wgrad(dy=dkv[:, c:], ldy=2 * c, n=c, x0=self._ctx_bf, c0=dctx, m=b * L, dw=self.g(bl + "/attn2/to_v/kernel"))
@@ -715,7 +727,8 @@ class UNet:
         qkv = t["qkv"]
         dqkv = A.alloc((m, 3 * c), BF16)
         ops.attention_bwd(qkv, qkv[:, c:], qkv[:, 2 * c:], t["ao1"], d_ao, t["lse1"], delta, dqkv, dqkv[:, c:],
-                          dqkv[:, 2 * c:], b, heads, hw, hw, 3 * c, 3 * c, 3 * c, c, c, 3 * c, 3 * c, 3 * c)
+                          dqkv[:, 2 * c:], b, heads, hw, hw, 3 * c, 3 * c, 3 * c, c, c, 3 * c, 3 * c, 3 * c,
+                          **_head_dim_kw(c, heads))
         for i, nm in enumerate(("to_q", "to_k", "to_v")):
             ops.wgrad(dy=dqkv[:, i * c:], ldy=3 * c, n=c, x0=t["ln1"], c0=c, m=m, dw=self.g(f"{bl}/attn1/{nm}/kernel"))
         ops.igemm(a0=dqkv, c0=3 * c, wt=self.wd[bl + "/attn1/qkv"], n=c, m=m, out_bf16=d_ln)   # one GEMM over K = 3C

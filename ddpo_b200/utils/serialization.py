@@ -28,6 +28,10 @@ StableParams = namedtuple("StableParams", "vae_params unet_params")
 MODEL_CONFIGS = {
     "stabilityai/stable-diffusion-2-base": "SD2_BASE",
     "flax/stable-diffusion-2-1": "SD2_BASE",
+    # SD1.x: 8 heads at every level (head dims 40, 80, 160), 768-wide CLIP-L context; the reference's default model
+    "duongna/stable-diffusion-v1-4-flax": "SD1",
+    "CompVis/stable-diffusion-v1-4": "SD1",
+    "runwayml/stable-diffusion-v1-5": "SD1",
     "tiny": "TINY",
     "small": "SMALL",
 }
@@ -37,7 +41,7 @@ def unet_config_for(pretrained_model):
     name = MODEL_CONFIGS.get(pretrained_model)
     if name is None:
         raise ValueError(f"[ utils/serialization ] no U-Net architecture registered for {pretrained_model!r}; known: "
-                         f"{sorted(MODEL_CONFIGS)} (SD1.x head dims 40/80/160 are not built, see DESIGN.md)")
+                         f"{sorted(MODEL_CONFIGS)}")
     return getattr(unet_spec, name)
 
 

@@ -195,9 +195,13 @@ int ddpo_dense_small_grouped(const float* x, const float* params_base, float* y_
                              int total_ctas, int batch, int k, void* stream);
 
 /* ---------------------------------------------------------------- attention --------
- * FlaxAttention core (3P diffusers attention_flax.py): softmax(Q K^T d^-0.5) V, head_dim 64. */
+ * FlaxAttention core (3P diffusers attention_flax.py): softmax(Q K^T d^-0.5) V with d = head_dim, which must be 40,
+ * 64, 80 or 160 (SD2: 64 everywhere; SD1.x: 40, 80, 160); any other value is DDPO_ERR_INVALID.
+ * Head h of q, k, v and out sits at columns [h*d, h*d + d).  Every bf16 pointer must be 16-byte aligned and every
+ * row pitch a multiple of 8 elements (16 bytes) and at least heads*d; otherwise DDPO_ERR_INVALID and nothing is
+ * written.  Only the d real columns of each head are written. */
 typedef struct {
-  const void* q;  /* bf16 [batch, nq, ldq], head h at columns [h*64, h*64+64) */
+  const void* q;  /* bf16 [batch, nq, ldq], head h at columns [h*d, h*d + d) */
   const void* k;  /* bf16 [batch, nk, ldk] */
   const void* v;  /* bf16 [batch, nk, ldv] */
   void* out;      /* bf16 [batch, nq, ldo] */
@@ -226,7 +230,9 @@ typedef struct {
 int64_t ddpo_wgrad_workspace_floats(const ddpo_wgrad_args* a);
 int ddpo_wgrad(const ddpo_wgrad_args* a, void* stream);
 
-/* attention backward (dQ, dK, dV; deterministic two-kernel scheme), see csrc/attention_bwd.cu */
+/* attention backward (dQ, dK, dV; deterministic two-kernel scheme), see csrc/attention_bwd.cu.  Head dims, column
+ * layout and alignment rules as for ddpo_attention_fwd (they apply to out, dout, dq, dk and dv too); the scale is
+ * head_dim^-0.5. */
 typedef struct {
   const void* q; const void* k; const void* v; const void* out; const void* dout; /* bf16 */
   const float* lse;  /* [batch, heads, nq] from the forward */
