@@ -122,6 +122,8 @@ SIGNATURES = {
     "ddpo_optim_workspace_bytes": (i64, []),
     "ddpo_grad_sumsq": (i32, [vp, i64, vp, vp, vp]),
     "ddpo_clip_adamw": (i32, [vp, vp, vp, vp, i64, vp, f32, f32, f32, f32, f32, f32, f32, i32, vp, vp]),
+    "ddpo_adafactor_plan": (i32, [i32, vp, vp, vp, i64, i32, vp, i64, vp, vp]),
+    "ddpo_clip_adafactor": (i32, [vp, vp, vp, i64, i64, vp, vp, vp, i64, vp, f32, f32, f32, f32, i32, vp, vp]),
 }
 
 _lib = None

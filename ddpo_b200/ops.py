@@ -5,6 +5,7 @@ torch is used for device memory and streams only; every arithmetic op below runs
 """
 import ctypes as C
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -367,7 +368,8 @@ def attention_bwd(q, k, v, out, dout, lse, delta, dq, dk, dv, batch, heads, nq, 
 
 _CIW_WS = {}
 _KERNELS_PER_CALL.update({"attention_bwd": 3, "colsum_cast": 2, "conv_out_bwd": 3, "conv_in_wgrad": 2,
-                          "dense_small_bwd": 3, "grad_sumsq": 2, "wgrad": 2, "colsum_bf16": 2})
+                          "dense_small_bwd": 3, "grad_sumsq": 2, "wgrad": 2, "colsum_bf16": 2,
+                          "clip_adafactor": 5})
 _COLSUM_WS = {}
 
 
@@ -472,6 +474,74 @@ def clip_adamw(params, grad_acc, mu, nu, sumsq, grad_scale, max_norm, lr, b1, b2
                                              float(grad_scale), float(max_norm), float(lr), float(b1), float(b2),
                                              float(eps), float(wd), int(step), _p(norm_out), _stream()),
          float(params.numel()) * 24, _e)
+
+
+class AdafactorPlan:
+    """Output of the host planner ``ddpo_adafactor_plan``: which tensors are factored, the layout of the Adafactor
+    state (optax's ``v_row``/``v_col``/``v``, leaf by leaf, in tensor order) and the tiling of the flat buffer.
+    ``host`` is the plan as int64 words; ``tensors`` [T, 12] and ``tiles`` [L, 9] are views of its records (field
+    order in ``csrc/adafactor.cu``)."""
+    T_WORDS, L_WORDS = 12, 9
+
+    def __init__(self, host, info, shapes, n, state_floats, workspace_floats):
+        self.host, self.shapes, self.n = host, shapes, n
+        self.state_floats, self.workspace_floats = state_floats, workspace_floats
+        self.kinds = [int(k) for k in info[:, 0]]          # 0 unfactored, 1 v_row over dim -2, 2 v_row over dim -1
+        self.state_offsets = [(int(a), int(b)) for a, b in info[:, 1:]]
+        nt, nl = int(host[2]), int(host[3])
+        self.tensors = host[8:8 + nt * self.T_WORDS].reshape(nt, self.T_WORDS)
+        self.tiles = host[8 + nt * self.T_WORDS:8 + nt * self.T_WORDS + nl * self.L_WORDS].reshape(nl, self.L_WORDS)
+        self._dev = {}
+
+    def device_copy(self, device):
+        d = self._dev.get(device)
+        if d is None:
+            d = self._dev[device] = torch.from_numpy(self.host).to(device)
+        return d
+
+    def state_shapes(self, t):
+        """optax's state leaves of tensor t: {"v_row": shape, "v_col": shape} or {"v": shape}"""
+        s, k = tuple(self.shapes[t]), self.kinds[t]
+        if k == 0:
+            return {"v": s}
+        over_rows, over_cols = s[:-1], s[:-2] + s[-1:]
+        return {"v_row": over_rows, "v_col": over_cols} if k == 1 else {"v_row": over_cols, "v_col": over_rows}
+
+    def state_views(self, state):
+        """per tensor, the views of the flat state buffer named as optax names them"""
+        out = []
+        for t in range(len(self.shapes)):
+            d = {}
+            for (name, shape), off in zip(self.state_shapes(t).items(), self.state_offsets[t]):
+                d[name] = state[off:off + int(np.prod(shape))].view(*shape)
+            out.append(d)
+        return out
+
+
+def adafactor_plan(tensors, n, min_dim_size_to_factor=128):
+    """Host-only planner.  ``tensors``: [(offset, shape)] views of the flat n-float buffer, ascending offsets."""
+    offs = np.array([int(o) for o, _ in tensors], np.int64)
+    nd = np.array([len(s) for _, s in tensors], np.int32)
+    dims = np.array([int(d) for _, s in tensors for d in s], np.int64)
+    sizes = np.zeros(3, np.int64)
+    info = np.zeros((len(tensors), 3), np.int64)
+    args = (len(tensors), offs.ctypes.data, nd.ctypes.data, dims.ctypes.data, int(n), int(min_dim_size_to_factor))
+    check(lib().ddpo_adafactor_plan(*args, None, 0, sizes.ctypes.data, None), "adafactor_plan")
+    host = np.zeros(int(sizes[0]), np.int64)
+    check(lib().ddpo_adafactor_plan(*args, host.ctypes.data, host.size, sizes.ctypes.data, info.ctypes.data),
+          "adafactor_plan")
+    return AdafactorPlan(host, info, [tuple(int(d) for d in s) for _, s in tensors], int(n), int(sizes[1]), int(sizes[2]))
+
+
+def clip_adafactor(params, grad_acc, state, plan, workspace, sumsq, grad_scale, max_norm, lr, wd, step, norm_out=None):
+    for t, nm in ((params, "params"), (grad_acc, "grad_acc"), (state, "state"), (workspace, "workspace")):
+        _chk(t, torch.float32, nm)
+    assert grad_acc.numel() == params.numel()
+    _e = _ev()
+    _run("clip_adafactor", lib().ddpo_clip_adafactor(
+        _p(params), _p(grad_acc), _p(state), state.numel(), params.numel(), plan.host.ctypes.data,
+        _p(plan.device_copy(params.device)), _p(workspace), workspace.numel(), _p(sumsq), float(grad_scale),
+        float(max_norm), float(lr), float(wd), int(step), _p(norm_out), _stream()), float(params.numel()) * 28, _e)
 
 
 # --------------------------------------------------------------------- RWR -------

@@ -32,7 +32,7 @@ import torch
 from .. import ops, training, utils
 from ..diffusers_patch import DDIMScheduler
 from ..training import distributed
-from ..training.policy_gradient import AccumulatingTrainState, AdamWConfig, train_step
+from ..training.policy_gradient import AccumulatingTrainState, AdafactorConfig, AdamWConfig, train_step
 from ..utils.stat_tracking import PerPromptStatTracker
 
 
@@ -273,10 +273,15 @@ def main(argv=None, models=None, max_epochs=None, save_last=True):
 
     # ------------------------------- optimizer --------------------------------#
     print("initializing train state...")
-    if args.optimizer != "adamw":
-        raise NotImplementedError("only optimizer=adamw is built (adafactor is out of scope, DESIGN.md §6)")
-    tx = AdamWConfig(learning_rate=args.learning_rate, b1=args.beta1, b2=args.beta2, eps=args.epsilon,
-                     weight_decay=args.weight_decay, max_grad_norm=args.max_grad_norm)                     # :130-150
+    optimizers = {                                                                                         # :130-150
+        "adamw": lambda: AdamWConfig(learning_rate=args.learning_rate, b1=args.beta1, b2=args.beta2, eps=args.epsilon,
+                                     weight_decay=args.weight_decay, max_grad_norm=args.max_grad_norm),
+        "adafactor": lambda: AdafactorConfig(learning_rate=args.learning_rate, weight_decay=args.weight_decay,
+                                             max_grad_norm=args.max_grad_norm),
+    }
+    if args.optimizer not in optimizers:
+        raise ValueError(f"optimizer={args.optimizer!r}: must be one of {', '.join(optimizers)}")
+    tx = optimizers[args.optimizer]()
     state = AccumulatingTrainState(step=0, apply_fn=pipeline.unet, params=params["unet"], tx=tx, n_acc=0)  # :156-164
 
     timer = utils.Timer()

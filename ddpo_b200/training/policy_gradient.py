@@ -20,7 +20,7 @@ parallel ``lax.pmean(grad)`` (:141) becomes ONE NCCL all-reduce of that buffer p
 (the mean is linear, so reducing the accumulated sum equals reducing every micro-step).
 """
 from dataclasses import dataclass
-from typing import Any, Dict, Optional
+from typing import Any, Dict, Union
 
 import torch
 
@@ -43,12 +43,25 @@ class AdamWConfig:
     max_grad_norm: float = 1.0
 
 
+@dataclass
+class AdafactorConfig:
+    """optax.chain(clip_by_global_norm(max_grad_norm), adafactor(learning_rate, weight_decay_rate=weight_decay))
+    hyper-parameters, every other adafactor argument at its optax default (reference pipeline/policy_gradient.py:132-150).
+    As in optax, the weight decay is added after the learning-rate scale: each update shrinks p by weight_decay * p."""
+    learning_rate: float = 1e-5
+    weight_decay: float = 1e-4
+    max_grad_norm: float = 1.0
+    min_dim_size_to_factor: int = 128
+
+
 class AccumulatingTrainState:
     """Accumulates gradients over several ``train_step`` calls and applies them when ``do_update``
-    (reference :13-57).  ``params`` / ``grad_acc`` are the U-Net's flat fp32 buffers."""
+    (reference :13-57).  ``params`` / ``grad_acc`` are the U-Net's flat fp32 buffers.  ``tx`` picks the optimizer:
+    AdamW keeps ``mu`` (bf16) and ``nu`` (fp32) over the whole buffer; Adafactor keeps only its factored second
+    moments, one flat fp32 ``state`` laid out by the host planner (``adafactor_leaves`` names its per-tensor views)."""
 
-    def __init__(self, *, step=0, apply_fn: UNet, params=None, tx: Optional[AdamWConfig] = None, opt_state=None,
-                 grad_acc=None, n_acc=0):
+    def __init__(self, *, step=0, apply_fn: UNet, params=None, tx: Union[AdamWConfig, AdafactorConfig, None] = None,
+                 opt_state=None, grad_acc=None, n_acc=0):
         self.step = int(step)
         self.apply_fn = apply_fn
         apply_fn.enable_training()
@@ -57,7 +70,13 @@ class AccumulatingTrainState:
         self.grad_acc = apply_fn.grads
         self.n_acc = int(n_acc)
         dev = self.params.device
-        if opt_state is None:
+        if isinstance(self.tx, AdafactorConfig):
+            self._plan = ops.adafactor_plan(list(apply_fn.table.values()), self.params.numel(),
+                                            self.tx.min_dim_size_to_factor)
+            self._af_ws = torch.empty(self._plan.workspace_floats, dtype=torch.float32, device=dev)
+            if opt_state is None:
+                opt_state = {"count": 0, "state": torch.zeros(self._plan.state_floats, dtype=torch.float32, device=dev)}
+        elif opt_state is None:
             opt_state = {"count": 0, "mu": torch.zeros(self.params.numel(), dtype=torch.bfloat16, device=dev),
                          "nu": torch.zeros(self.params.numel(), dtype=torch.float32, device=dev)}
         self.opt_state = opt_state
@@ -68,6 +87,11 @@ class AccumulatingTrainState:
     @classmethod
     def create(cls, *, apply_fn, params=None, tx=None, **kw):
         return cls(step=0, apply_fn=apply_fn, params=params, tx=tx, **kw)
+
+    def adafactor_leaves(self):
+        """Adafactor only: parameter name -> {"v_row", "v_col"} or {"v"} views of the state, shaped as optax's."""
+        views = self._plan.state_views(self.opt_state["state"])
+        return dict(zip(self.apply_fn.table, views))
 
     def apply_gradients(self, *, grads=None, do_update: bool, n_micro: int = 1, **kwargs):
         """``grads`` is accepted for signature parity; the backward pass has already added this step's
@@ -80,9 +104,14 @@ class AccumulatingTrainState:
         ops.grad_sumsq(self.grad_acc, self._ws, self._sumsq)
         self.opt_state["count"] += 1
         c = self.tx
-        ops.clip_adamw(self.params, self.grad_acc, self.opt_state["mu"], self.opt_state["nu"], self._sumsq,
-                       distributed.grad_scale(self.n_acc, world), c.max_grad_norm, c.learning_rate, c.b1, c.b2, c.eps, c.weight_decay,
-                       self.opt_state["count"], norm_out=self.last_grad_norm)
+        if isinstance(c, AdafactorConfig):
+            ops.clip_adafactor(self.params, self.grad_acc, self.opt_state["state"], self._plan, self._af_ws, self._sumsq,
+                               distributed.grad_scale(self.n_acc, world), c.max_grad_norm, c.learning_rate, c.weight_decay,
+                               self.opt_state["count"], norm_out=self.last_grad_norm)
+        else:
+            ops.clip_adamw(self.params, self.grad_acc, self.opt_state["mu"], self.opt_state["nu"], self._sumsq,
+                           distributed.grad_scale(self.n_acc, world), c.max_grad_norm, c.learning_rate, c.b1, c.b2, c.eps,
+                           c.weight_decay, self.opt_state["count"], norm_out=self.last_grad_norm)
         self.apply_fn.refresh_weights()
         self.step += 1
         self.n_acc = 0

@@ -350,6 +350,29 @@ int ddpo_clip_adamw(float* params, float* grad_acc, void* mu_bf16, float* nu, in
                     float grad_scale, float max_norm, float lr, float b1, float b2, float eps, float weight_decay,
                     int step, float* norm_out, void* stream);
 
+/* optax.chain(clip_by_global_norm, adafactor(lr, weight_decay_rate=wd)) at optax's other defaults (momentum None,
+ * decay_rate 0.8, eps 1e-30, clipping_threshold 1, multiply_by_parameter_scale) + the same apply_gradients
+ * (pipeline/policy_gradient.py:132-150).
+ * ddpo_adafactor_plan (host only, no device needed): tensor t has ndims[t] dims (taken in order from `dims`) and
+ * starts at offsets[t] of the flat n-float buffer; offsets ascend and tensors do not overlap.  A tensor is factored as
+ * optax decides (ndim >= 2 and second-largest dim >= min_dim_size_to_factor); its two largest dims must then be its
+ * last two, its last dim a multiple of 4 and its offset a multiple of 4, else DDPO_ERR_INVALID.  sizes[3] receives the
+ * plan's int64 words, the state floats and the workspace floats; tensor_info[ntensors][3] (may be NULL) receives per
+ * tensor the kind (0 unfactored, 1 factored with v_row over the second-last dim, 2 factored with v_row over the last
+ * dim) and the state offsets of v_row and v_col, or of v and -1.  State is optax's v_row, v_col / v, leaf by leaf, in
+ * tensor order.  With plan == NULL only the sizes are computed.  On error nothing is written.
+ * ddpo_clip_adafactor: plan_host and plan_dev are the same plan in host and device memory; params and grad_acc
+ * 16-byte aligned; state zero-initialised before step 1; step = 1 + number of earlier updates.  The workspace starts
+ * with [ntensors][2] floats: each tensor's clip denominator max(1, rms(u)) and parameter scale.  On an argument error
+ * nothing is written. */
+int ddpo_adafactor_plan(int ntensors, const int64_t* offsets, const int32_t* ndims, const int64_t* dims, int64_t n,
+                        int min_dim_size_to_factor, int64_t* plan, int64_t plan_words, int64_t* sizes,
+                        int64_t* tensor_info);
+int ddpo_clip_adafactor(float* params, float* grad_acc, float* state, int64_t state_floats, int64_t n,
+                        const int64_t* plan_host, const int64_t* plan_dev, float* workspace, int64_t workspace_floats,
+                        const float* sumsq_dev, float grad_scale, float max_norm, float lr, float weight_decay, int step,
+                        float* norm_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
