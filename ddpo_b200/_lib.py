@@ -124,6 +124,11 @@ SIGNATURES = {
     "ddpo_clip_adamw": (i32, [vp, vp, vp, vp, i64, vp, f32, f32, f32, f32, f32, f32, f32, i32, vp, vp]),
     "ddpo_adafactor_plan": (i32, [i32, vp, vp, vp, i64, i32, vp, i64, vp, vp]),
     "ddpo_clip_adafactor": (i32, [vp, vp, vp, i64, i64, vp, vp, vp, i64, vp, f32, f32, f32, f32, i32, vp, vp]),
+    "ddpo_resample_u8": (i32, [vp, i32, i32, i32, i32, i32, i32, vp, vp, i32, vp, vp]),
+    "ddpo_clip_normalize_u8": (i32, [vp, i32, i32, i32, i32, i32, i32, vp, vp]),
+    "ddpo_pair_stats_u8": (i32, [vp, i32, i32, i32, i32, vp, vp]),
+    "ddpo_feature_angles": (i32, [vp, i32, i32, i32, vp, vp]),
+    "ddpo_scaled_cosine": (i32, [vp, vp, i32, i32, f32, vp, vp]),
 }
 
 _lib = None

@@ -609,6 +609,70 @@ def image_to_uint8(img, out_u8):
     _run("image_to_uint8", lib().ddpo_image_to_uint8(_p(img), _p(out_u8), img.numel(), _stream()), 0.0, _e)
 
 
+# ------------------------------------------------- image-symmetry / consistency rewards -------
+def resample_u8(src, transform, axis, table_host, table_dev, dst):
+    """one pass of Pillow's bicubic resize (``include/ddpo_b200.h``); ``table_host`` int32 numpy and ``table_dev`` its
+    device copy (``clip_vision.resample_table``)"""
+    _chk(src, torch.uint8, "src")
+    _chk(dst, torch.uint8, "dst")
+    _chk(table_dev, torch.int32, "table")
+    assert table_host.dtype == np.int32 and table_host.flags.c_contiguous and tuple(table_dev.shape) == table_host.shape
+    b, h, w, c = src.shape
+    n_out = table_host.shape[0]
+    th, tw = (w, h) if transform in (2, 4) else (h, w)
+    assert c == 3 and tuple(dst.shape) == ((b, th, n_out, 3) if axis == 0 else (b, n_out, tw, 3)), (src.shape, dst.shape)
+    _e = _ev()
+    _run("resample_u8", lib().ddpo_resample_u8(_p(src), b, h, w, int(transform), int(axis), n_out,
+                                               table_host.ctypes.data, _p(table_dev), table_host.shape[1] - 2, _p(dst),
+                                               _stream()), float(dst.numel() + src.numel()), _e)
+
+
+def clip_normalize_u8(src, top, left, out):
+    """CLIP rescale + normalise of the ``size`` x ``size`` crop at (top, left) -> fp32 NHWC ``out``"""
+    _chk(src, torch.uint8, "src")
+    _chk(out, torch.float32, "out")
+    b, h, w, _ = src.shape
+    size = out.shape[1]
+    assert tuple(out.shape) == (b, size, size, 3)
+    _e = _ev()
+    _run("clip_normalize_u8", lib().ddpo_clip_normalize_u8(_p(src), b, h, w, int(top), int(left), size, _p(out),
+                                                           _stream()), float(out.numel()) * 5, _e)
+
+
+def pair_stats_u8(src, transform, out):
+    """per image against its mirror (1) or 180-degree rotation (3): int64 [B, 4] = (sum of uint8-wrapped squared
+    differences, sum a, sum a^2, sum a T(a))"""
+    _chk(src, torch.uint8, "src")
+    _chk(out, torch.int64, "out")
+    b, h, w, _ = src.shape
+    assert tuple(out.shape) == (b, 4)
+    _e = _ev()
+    _run("pair_stats_u8", lib().ddpo_pair_stats_u8(_p(src), b, h, w, int(transform), _p(out), _stream()),
+         float(src.numel()) * 2, _e)
+
+
+def feature_angles(feats, variants, out):
+    """feats fp32 [variants * n, dim] -> out [n]: mean over variants >= 1 of the angle (degrees) to variant 0"""
+    _chk(feats, torch.float32, "feats")
+    _chk(out, torch.float32, "out")
+    n = out.numel()
+    assert feats.dim() == 2 and feats.shape[0] == variants * n
+    _e = _ev()
+    _run("feature_angles", lib().ddpo_feature_angles(_p(feats), int(variants), n, feats.shape[1], _p(out), _stream()),
+         float(feats.numel()) * 4, _e)
+
+
+def scaled_cosine(img, txt, logit_scale, out):
+    """out[i] = exp(logit_scale) cos(img[i], txt[i])"""
+    _chk(img, torch.float32, "img")
+    _chk(txt, torch.float32, "txt")
+    _chk(out, torch.float32, "out")
+    assert img.shape == txt.shape and img.dim() == 2 and out.numel() == img.shape[0]
+    _e = _ev()
+    _run("scaled_cosine", lib().ddpo_scaled_cosine(_p(img), _p(txt), img.shape[0], img.shape[1], float(logit_scale),
+                                                   _p(out), _stream()), float(img.numel()) * 8, _e)
+
+
 def vae_image_to_nchw(img_nhwc, out_nchw):
     _chk(img_nhwc, torch.float32, "images")
     _chk(out_nchw, torch.float32, "out")

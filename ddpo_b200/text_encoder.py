@@ -38,6 +38,8 @@ class CLIPTextConfig:
 SD2_TEXT = CLIPTextConfig()
 SD1_TEXT = CLIPTextConfig(hidden_size=768, intermediate_size=3072, num_hidden_layers=12, num_attention_heads=12,
                           hidden_act="quick_gelu")
+CLIP_B32_TEXT = CLIPTextConfig(hidden_size=512, intermediate_size=2048, num_hidden_layers=12, num_attention_heads=8,
+                               hidden_act="quick_gelu")     # openai/clip-vit-base-patch32 (the consistency reward)
 TEXT_TINY = CLIPTextConfig(vocab_size=1000, hidden_size=128, intermediate_size=512, num_hidden_layers=2,
                            num_attention_heads=2)
 TEXT_TINY_QUICK = CLIPTextConfig(vocab_size=1000, hidden_size=192, intermediate_size=256, num_hidden_layers=1,

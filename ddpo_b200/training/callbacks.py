@@ -2,11 +2,17 @@
 ``callback_fns[name]() -> fn(images f32 NHWC in [0,1] [N,H,W,3], prompts, metadata) -> (scores, info)``.
 ``jpeg`` / ``neg_jpeg`` (:143-163, JPEG q=95 size in kB via PIL, ``hdf5.py:25-37``) and ``arange`` (:347-354)
 are real; the model-based rewards (aesthetic CLIP+MLP, LLaVA over HTTP) need weights / a server that do not
-exist offline and are provided as cached-score stubs (BASELINE.json configs 3 and 5)."""
+exist offline and are provided as cached-score stubs (BASELINE.json configs 3 and 5).  The image-symmetry rewards
+(``mirror``, ``mirror_corr``, ``rotational``, ``rotational_corr``, ``thumbnail``, :166-344) and ``consistency``
+(:122-140) run on the GPU kernels: the images go to the device once as uint8 and every transform, resample and reduction
+happens there (``csrc/image_rewards.cu``); their CLIP towers are random-init, seeded as ``aesthetic``'s."""
 import io
 import random
 
 import numpy as np
+import torch
+
+from .. import clip_vision as CV, ops
 
 
 def encode_jpeg(x, quality=95):
@@ -161,6 +167,126 @@ def vae_fn(devices=None, dtype="float32", jit=True, encoder=None, pretrained_mod
     return _fn
 
 
+def _device(device=None):
+    if device is not None:
+        return torch.device(device)
+    return torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
+
+
+def _image_bytes(images, device):
+    """the reference's ``(image * 255).astype(np.uint8)`` (:181) for float images, uint8 as it is; one copy to the device"""
+    x = np.asarray(images)
+    if x.dtype != np.uint8:
+        x = (x * 255).astype(np.uint8)
+    assert x.ndim == 4 and x.shape[-1] == 3, x.shape
+    return torch.from_numpy(np.ascontiguousarray(x)).to(device)
+
+
+def _pair_stats(images, transform, device):
+    """per image, exact integer sums against its mirror / 180-degree rotation: uint64 [N, 4] (wrapped squared difference,
+    sum a, sum a^2, sum a T(a)) and the number of bytes per image"""
+    u8 = _image_bytes(images, device)
+    st = torch.empty(len(u8), 4, dtype=torch.int64, device=device)
+    ops.pair_stats_u8(u8, transform, st)
+    return st.cpu().numpy().view(np.uint64), u8[0].numel()
+
+
+def _wrapped_mse(images, transform, device):
+    """``((a - T a) ** 2).mean(axis=(1, 2, 3))`` of uint8 arrays, numpy's uint8 wrap included: the float64 mean of
+    integers below 2**53 is exactly their sum over the count"""
+    st, n = _pair_stats(images, transform, device)
+    return st[:, 0].astype(np.float64) / n
+
+
+def mirror_symmetry_fn(devices=None, jit=False, device=None):
+    """Reference :244-260: ``-((pils - mirrored) ** 2).mean(axis=(1, 2, 3))`` on uint8 arrays, float64 [N].  The
+    subtraction and the square wrap modulo 256, as numpy's uint8 arithmetic does in the reference."""
+    dev = _device(device)
+
+    def _fn(images, prompts, metadata):
+        return -_wrapped_mse(images, CV.MIRROR, dev), {}
+    _fn.accepts_uint8 = True
+    return _fn
+
+
+def rotational_correlation_fn(devices=None, jit=False, device=None):
+    """Reference :216-241: the same wrapped mean squared difference against ``pil.rotate(180)``, negated; float64 [N]."""
+    dev = _device(device)
+
+    def _fn(images, prompts, metadata):
+        return -_wrapped_mse(images, CV.ROT180, dev), {}
+    _fn.accepts_uint8 = True
+    return _fn
+
+
+def mirror_correlation_fn(devices=None, jit=False, device=None):
+    """Reference :268-292: minus the Pearson correlation of an image's bytes with its mirror's, float32 [N].  Computed
+    exactly from integer sums (the reference's float32 cov differs from it by ~1e-7).  An image of zero variance (a flat
+    image, e.g. all black) scores NaN, as 0 / 0 does in the reference."""
+    dev = _device(device)
+
+    def _fn(images, prompts, metadata):
+        st, n = _pair_stats(images, CV.MIRROR, dev)
+        out = np.empty(len(st), np.float32)
+        for i, (_, sa, saa, sab) in enumerate(st.tolist()):
+            den = n * saa - sa * sa          # the mirror is a permutation: sum b = sum a, sum b^2 = sum a^2
+            out[i] = np.nan if den == 0 else -(n * sab - sa * sa) / den
+        return out, {}
+    _fn.accepts_uint8 = True
+    return _fn
+
+
+def _angle_reward(variants, images, device):
+    """-mean over variants >= 1 of the angle (degrees) between the CLIP features of variant 0 and variant v (reference
+    :196-211, :327-342); ``variants`` are functions of the uint8 device batch to the tower's feature rows"""
+    u8 = _image_bytes(images, device)
+    feats = torch.cat([v(u8) for v in variants])
+    out = torch.empty(len(u8), dtype=torch.float32, device=device)
+    ops.feature_angles(feats, len(variants), out)
+    return -out.cpu().numpy(), {}
+
+
+def rotational_symmetry_fn(devices=None, jit=True, rng=0, cfg=None, device=None):
+    """Reference :166-213: CLIP ViT-L/14 features of ``pil.rotate(0 / 90 / 180 / 270)``, minus the mean angle between
+    the original's and each rotation's; float32 [N].  Square images only (Pillow rotates others through its affine path)."""
+    dev = _device(device)
+    tower = CV.CLIPImageTower(cfg or CV.VIT_L14, device=dev, seed=int(rng))
+    variants = [lambda u8, t=t: tower.features(u8, t) for t in (CV.IDENTITY, CV.ROT90, CV.ROT180, CV.ROT270)]
+
+    def _fn(images, prompts, metadata):
+        return _angle_reward(variants, images, dev)
+    _fn.accepts_uint8 = True
+    return _fn
+
+
+def thumbnail_fn(devices=None, jit=True, rng=0, cfg=None, device=None):
+    """Reference :295-344: CLIP ViT-L/14 features of the image and of its bicubic thumbnails at 1/4, 1/8 and 1/16 size
+    (``pil.resize``), minus the mean angle between the original's and each thumbnail's; float32 [N]."""
+    dev = _device(device)
+    tower = CV.CLIPImageTower(cfg or CV.VIT_L14, device=dev, seed=int(rng))
+
+    def thumb(d):
+        return lambda u8: tower.features(CV.resize_u8(u8, u8.shape[2] // d, u8.shape[1] // d))
+    variants = [tower.features] + [thumb(d) for d in (4, 8, 16)]
+
+    def _fn(images, prompts, metadata):
+        return _angle_reward(variants, images, dev)
+    _fn.accepts_uint8 = True
+    return _fn
+
+
+def consistency_fn(devices=None, jit=False, rng=0, model=None, device=None):
+    """Reference :122-140: CLIP ViT-B/32 ``logits_per_image.diagonal()[:, None]`` of each image with its own prompt,
+    float32 [N, 1] (``clip_vision.CLIPConsistency``)."""
+    dev = _device(device)
+    model = model or CV.CLIPConsistency(device=dev, seed=int(rng))
+
+    def _fn(images, prompts, metadata):
+        return model(_image_bytes(images, dev), prompts)[:, None], {}
+    _fn.accepts_uint8 = True
+    return _fn
+
+
 def evaluate_callbacks(fns, images, prompts, metadata):
     if type(prompts[0]) == list:
         prompts = [random.choice(p) for p in prompts]
@@ -179,4 +305,10 @@ callback_fns = {
     "llava_vqa": _cached_score_stub("llava_vqa", False),     # callbacks.py:401-461 needs the LLaVA server; offline stub
     "vqa": _cached_score_stub("vqa", True),
     "vae": vae_fn,
+    "consistency": consistency_fn,
+    "rotational": rotational_symmetry_fn,
+    "rotational_corr": rotational_correlation_fn,
+    "mirror": mirror_symmetry_fn,
+    "mirror_corr": mirror_correlation_fn,
+    "thumbnail": thumbnail_fn,
 }

@@ -373,6 +373,30 @@ int ddpo_clip_adafactor(float* params, float* grad_acc, float* state, int64_t st
                         const float* sumsq_dev, float grad_scale, float max_norm, float lr, float weight_decay, int step,
                         float* norm_out, void* stream);
 
+/* ------------------------------------------------ image-symmetry / consistency rewards -----
+ * Reference ddpo/training/callbacks.py:122-140 (consistency), 166-213 (rotational), 216-241 (rotational_corr),
+ * 244-260 (mirror), 268-292 (mirror_corr), 295-344 (thumbnail).  Images are uint8 NHWC RGB [batch, h, w, 3].
+ * Transforms, read in place by the first pass: ImageOps.mirror, and Pillow's rotate(90 / 180 / 270) fast paths
+ * (transposes; 90 and 270 only for square images -- Pillow rotates other shapes through its affine path). */
+enum { DDPO_IMAGE_IDENTITY = 0, DDPO_IMAGE_MIRROR = 1, DDPO_IMAGE_ROT90 = 2, DDPO_IMAGE_ROT180 = 3, DDPO_IMAGE_ROT270 = 4 };
+/* One pass of Image.resize(BICUBIC, reducing_gap=None): axis 0 resamples the columns of the transformed image
+ * (dst [batch, th, n_out, 3]), axis 1 its rows (dst [batch, n_out, tw, 3]); (th, tw) = (h, w), swapped for 90 / 270.
+ * table [n_out][2 + ksize] int32 (xmin, n, then n of ksize 22-bit fixed-point weights), once in host and once in
+ * device memory; every entry must lie inside the input.  acc = 2^21 + sum(pixel * k), dst = clamp(acc >> 22, 0, 255). */
+int ddpo_resample_u8(const uint8_t* src, int batch, int h, int w, int transform, int axis, int n_out,
+                     const int32_t* table_host, const int32_t* table_dev, int ksize, uint8_t* dst, void* stream);
+/* out fp32 [batch, size, size, 3] = (double(float32(x) / 255) - CLIP mean) / CLIP std of the crop at (top, left) */
+int ddpo_clip_normalize_u8(const uint8_t* src, int batch, int h, int w, int top, int left, int size, float* out,
+                           void* stream);
+/* out [batch][4]: sum(((a - T a) mod 256)^2 mod 256), sum a, sum a^2, sum a * T(a) over all h * w * 3 bytes of each
+ * image; T is DDPO_IMAGE_MIRROR or DDPO_IMAGE_ROT180 */
+int ddpo_pair_stats_u8(const uint8_t* src, int batch, int h, int w, int transform, uint64_t* out, void* stream);
+/* feats fp32 [variants * n, dim] (row v * n + i: variant v of image i, variant 0 the original) -> out[n] fp32 = mean
+ * over v >= 1 of degrees(arccos(clip(cos(f_0, f_v), 0, 1))), in double */
+int ddpo_feature_angles(const float* feats, int variants, int n, int dim, float* out, void* stream);
+/* out[i] = exp(logit_scale) * cos(img[i], txt[i]) for fp32 [n, dim] rows, in double */
+int ddpo_scaled_cosine(const float* img, const float* txt, int n, int dim, float logit_scale, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
