@@ -4,21 +4,25 @@
 // pipeline_flax_stable_diffusion.py:219-224 / training/policy_gradient.py:87-102).  SD2 runs d = 64 at every level,
 // SD1.x (8 heads) runs d = 40, 80 and 160.
 //
-// The [B*h, N, N] score tensor XLA materialises never exists here.  One CTA owns a 128-query
-// tile of one (sample, head), two consumer warpgroups of 64 query rows each; K/V stream through a
-// 2-stage TMA ring in 128-key blocks (warp 8 is the producer).  At d = 80 and 160 the blocks have 64 keys: the wider O
-// accumulator leaves no registers for a 128-key score tile under the 168-register cap of a 288-thread CTA, and at
-// d = 160 two 128-key stages would not fit in shared memory.
+// The [B*h, N, N] score tensor XLA materialises never exists here.  One CTA owns a 128-query tile of one
+// (sample, head), two consumer warpgroups of 64 query rows each; K/V stream through a TMA ring of NST stages in 128-key
+// blocks (warp 8 is the producer).  At d = 80 and 160 the blocks have 64 keys: the wider O accumulator leaves no
+// registers for a 128-key score tile under the 168-register cap of a 288-thread CTA, and at d = 160 a 128-key ring
+// would not fit in shared memory.
 //   S_j   = Q K_j^T          wgmma m64nBKVk16 (both operands K-major in shared memory) -> registers
 //   P_j   = exp2((S_j - m) c)   in registers (a quad of threads holds a query row), bf16
 //   O     = O * alpha + P_j V_j   wgmma m64n64k16 per 64 columns, A = P from registers, B = V MN-major
-// normalised by the row sum at the end.  Keys past nk (TMA zero fill) and, with causal masking, keys
-// after the query are masked; key blocks entirely after a causal tile are skipped.
+// normalised by the row sum at the end.
+// Keys past nk (TMA zero fill) and, with causal masking, keys after the query are masked; key blocks entirely after a
+// causal tile are skipped.  Only a block that reaches past nk or the tile's first causal row runs the per-element mask:
+// the blocks of 4096-, 1024- and 256-token self-attention are all full.
 // The head dim is padded in shared memory to whole 64-column SW128 boxes (40 -> 64, 80 -> 128, 160 -> 192): each
 // tensor map's innermost extent is the real d, so TMA zero-fills columns [d, 64 * ceil(d / 64)) and the next head's
 // data never enters the tile.  The zero columns add nothing to Q K^T and give O columns that are not stored.  Padding
 // costs only wgmma work; the softmax (MUFU / issue), which bounds the kernel, is counted per score.
 // Fixed reduction order; no atomics.
+#include <type_traits>
+
 #include "common.cuh"
 #include "wgmma.cuh"
 
@@ -28,7 +32,7 @@ constexpr int AT_THREADS = 288;  // warps 0-7: two consumer warpgroups, warp 8: 
 constexpr int AT_BQ = 128;
 constexpr int AT_CHUNK = 64;      // head-dim columns per SW128 box (128 B rows)
 
-// Shared-memory plan of head dim D: Q | 2 stages x (K | V), each operand as D_PAD / 64 column chunks of SW128 tiles.
+// Shared-memory plan of head dim D: Q | NST stages x (K | V), each operand as D_PAD / 64 column chunks of SW128 tiles.
 template <int D>
 struct AtPlan {
   static constexpr int NCH = (D + AT_CHUNK - 1) / AT_CHUNK;  // 64-column chunks (padded head dim / 64)
@@ -38,8 +42,11 @@ struct AtPlan {
   static constexpr int STAGE = 2 * NCH * KV_CHUNK;           // K chunks | V chunks
   static constexpr int SMEM_Q = 0;
   static constexpr int SMEM_KV = NCH * Q_CHUNK;
-  static constexpr int SMEM_BAR = SMEM_KV + 2 * STAGE;
+  static constexpr int FIT = (227 * 1024 - 1280 - SMEM_KV) / STAGE;
+  static constexpr int NST = FIT < 4 ? FIT : 4;              // 4 stages; 3 at d = 160 (48 KB each)
+  static constexpr int SMEM_BAR = SMEM_KV + NST * STAGE;
   static constexpr int SMEM_TOTAL = SMEM_BAR + 256 + 1024;  // + alignment slack
+  static_assert(NST >= 2, "attention_fwd: shared memory plan has room for fewer than two K/V stages");
   static_assert(SMEM_TOTAL <= 227 * 1024, "attention_fwd: shared memory plan exceeds 227 KB");
 };
 
@@ -53,25 +60,78 @@ struct AttnArgs {
   float scale;
 };
 
+// Column col = 8 jj + 2 t4 + e of a score fragment takes the polynomial exponent when col % PERIOD == PERIOD - 1
+// (PERIOD = DDPO_EXP_POLY_FWD).  For an even PERIOD that divides 8 this holds only for e = 1 and only on lanes with
+// (2 t4 + 1) % PERIOD == PERIOD - 1, so the choice is a per-lane select instead of a divergent branch per element.
+static_assert(DDPO_EXP_POLY_FWD == 0 || (DDPO_EXP_POLY_FWD % 2 == 0 && 8 % DDPO_EXP_POLY_FWD == 0),
+              "attention_fwd: the polynomial period must be 0, 2, 4 or 8");
+
+// Online softmax of one key block for the thread's two query rows: S -> P as the bf16 A fragments of the P V wgmma (each
+// pair is packed as soon as it is computed, so the fp32 scores die early), returns the O rescale per row.
+// MASK: keys past nk and, when causal, after the row (rows row0 and row0 + 8) are excluded (the tail block past nk, the
+// causal diagonal); key 0 is always visible.
+template <int BKV, bool MASK>
+__device__ __forceinline__ void softmax_block(const float (&s)[BKV / 2], uint32_t (&pa)[BKV / 16][4], float (&m_run)[2],
+                                              float (&l_run)[2], float (&alpha)[2], int row0, int nk, int causal,
+                                              int kbase, int t4, bool poly_lane, float c) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int valid = (causal ? min(nk, row0 + 8 * h + 1) : nk) - kbase;
+    float mx4[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};  // max is exact: any grouping gives the same value
+#pragma unroll
+    for (int jj = 0; jj < BKV / 8; ++jj)
+#pragma unroll
+      for (int e = 0; e < 2; ++e)
+        if (!MASK || 8 * jj + 2 * t4 + e < valid) mx4[(jj & 1) * 2 + e] = fmaxf(mx4[(jj & 1) * 2 + e], s[4 * jj + 2 * h + e]);
+    float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+    const float m_new = fmaxf(m_run[h], mx);
+    alpha[h] = ex2_mufu((m_run[h] - m_new) * c);
+    const float mc = m_new * c;
+    float l_blk = 0.f;
+#pragma unroll
+    for (int jj = 0; jj < BKV / 8; ++jj) {
+      float pr[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float x = fmaf(s[4 * jj + 2 * h + e], c, -mc);
+        pr[e] = ex2_mufu(x);
+        if (DDPO_EXP_POLY_FWD > 0 && e == 1) {
+          const float pp = ex2_poly(x);
+          pr[e] = poly_lane ? pp : pr[e];
+        }
+        if (MASK && !(8 * jj + 2 * t4 + e < valid)) pr[e] = 0.f;
+        l_blk += pr[e];
+      }
+      pa[jj / 2][2 * (jj & 1) + h] = pack_bf16(pr[0], pr[1]);  // A fragment: rows r, r + 8 x keys 8 jj + 2 t4 + {0, 1}
+    }
+    l_run[h] = fmaf(l_run[h], alpha[h], l_blk);  // this thread's partial row sum (the quad is summed at the end)
+    m_run[h] = m_new;
+  }
+}
+
 template <int D>
 __global__ void __launch_bounds__(AT_THREADS, 1) attention_fwd_kernel(const __grid_constant__ AttnArgs p) {
   using P = AtPlan<D>;
-  constexpr int NCH = P::NCH, BKV = P::BKV;
+  constexpr int NCH = P::NCH, BKV = P::BKV, NST = P::NST;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + P::SMEM_BAR);
-  uint64_t* q_full = bars;        // 1
-  uint64_t* kv_full = bars + 1;   // [2]
-  uint64_t* kv_empty = bars + 3;  // [2] (one arrive per consumer warp)
+  uint64_t* q_full = bars;              // 1
+  uint64_t* kv_full = bars + 1;         // [NST]
+  uint64_t* kv_empty = bars + 1 + NST;  // [NST] (one arrive per consumer warp)
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // the warp index through a shuffle: the compiler then treats it, and the role branch, as warp-uniform (no divergent
+  // fallback paths around the softmax shuffles)
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * AT_BQ, head = blockIdx.y, b = blockIdx.z;
   const int k_end = p.causal ? min(p.nk, q0 + AT_BQ) : p.nk;
   const int nkb = (k_end + BKV - 1) / BKV;
 
   if (threadIdx.x == 0) {
     mbar_init(q_full, 1);
-    for (int i = 0; i < 2; ++i) {
+    for (int i = 0; i < NST; ++i) {
       mbar_init(&kv_full[i], 1);
       mbar_init(&kv_empty[i], 8);
     }
@@ -89,8 +149,8 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attention_fwd_kernel(const __gr
       for (int c = 0; c < NCH; ++c)
         tma_load_4d(smem + P::SMEM_Q + c * P::Q_CHUNK, &p.tmQ, q_full, c * AT_CHUNK, head, q0, b);
       for (int j = 0; j < nkb; ++j) {
-        const int st = j & 1;
-        mbar_wait(&kv_empty[st], ((j >> 1) & 1) ^ 1);
+        const int st = j % NST;
+        mbar_wait(&kv_empty[st], ((j / NST) & 1) ^ 1);
         uint8_t* sK = smem + P::SMEM_KV + st * P::STAGE;
         mbar_expect_tx(&kv_full[st], P::STAGE);
 #pragma unroll
@@ -105,15 +165,12 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attention_fwd_kernel(const __gr
   }
 
   // ------------------------------------------------------------ consumer warpgroups
-  // accumulator fragments: thread holds query rows rq[0] = .. + lane / 4 and rq[1] = rq[0] + 8, columns 8 j + 2 (lane & 3) + {0, 1}
+  // accumulator fragments: thread holds query rows row0 = .. + lane / 4 and row0 + 8, columns 8 j + 2 (lane & 3) + {0, 1}
   const int wg = warp >> 2;
   const int t4 = lane & 3;
-  int rq[2];
-  rq[0] = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-  rq[1] = rq[0] + 8;
-  int k_lim[2];  // keys [0, k_lim) are visible to the row (causal: j <= i; key 0 is always visible)
-#pragma unroll
-  for (int h = 0; h < 2; ++h) k_lim[h] = p.causal ? min(p.nk, rq[h] + 1) : p.nk;
+  const bool poly_lane = DDPO_EXP_POLY_FWD > 0 && (2 * t4 + 1) % (DDPO_EXP_POLY_FWD > 0 ? DDPO_EXP_POLY_FWD : 1) ==
+                                                      DDPO_EXP_POLY_FWD - 1;
+  const int row0 = q0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
   const float c = p.scale_log2e;
   float o[NCH][AT_CHUNK / 2];  // O columns 64 ch + ..
 #pragma unroll
@@ -122,76 +179,70 @@ __global__ void __launch_bounds__(AT_THREADS, 1) attention_fwd_kernel(const __gr
     for (int i = 0; i < AT_CHUNK / 2; ++i) o[ch][i] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
   const uint32_t q_addr = smem_u32(smem + P::SMEM_Q) + wg * (64 * 128);
-  mbar_wait(q_full, 0);
-  for (int j = 0; j < nkb; ++j) {
-    const int st = j & 1;
-    mbar_wait(&kv_full[st], (j >> 1) & 1);
-    const uint32_t k_addr = smem_u32(smem + P::SMEM_KV + st * P::STAGE), v_addr = k_addr + NCH * P::KV_CHUNK;
-    float s[BKV / 2];
-    wgmma_fence();
+  const uint32_t kv_base = smem_u32(smem + P::SMEM_KV);
+  float s[BKV / 2];
+  uint32_t pa[BKV / 16][4];
+
+  auto issue_s = [&](int st) {
+    const uint32_t k_addr = kv_base + st * P::STAGE;
 #pragma unroll
     for (int k = 0; k < NCH * AT_CHUNK / 16; ++k)  // 16 head-dim columns per instruction, 4 per 128-byte chunk row
       Wgmma<BKV>::template ss<0, 0>(s, gmma_desc(q_addr + (k / 4) * P::Q_CHUNK + (k % 4) * 32, 16, 1024),
                                     gmma_desc(k_addr + (k / 4) * P::KV_CHUNK + (k % 4) * 32, 16, 1024), k != 0);
     wgmma_commit();
-    wgmma_wait<0>();
-    const int kbase = j * BKV;
-    uint32_t pa[BKV / 16][4];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int valid = k_lim[h] - kbase;
-      float mx = -INFINITY;
-#pragma unroll
-      for (int jj = 0; jj < BKV / 8; ++jj)
-#pragma unroll
-        for (int e = 0; e < 2; ++e)
-          if (8 * jj + 2 * t4 + e < valid) mx = fmaxf(mx, s[4 * jj + 2 * h + e]);
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-      const float m_new = fmaxf(m_run[h], mx);
-      const float alpha = ex2_mufu((m_run[h] - m_new) * c);
-      const float mc = m_new * c;
-      float l_blk = 0.f;
-#pragma unroll
-      for (int jj = 0; jj < BKV / 8; ++jj)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int col = 8 * jj + 2 * t4 + e;
-          const float pr = col < valid ? ex2_sel<DDPO_EXP_POLY_FWD>(col, s[4 * jj + 2 * h + e] * c - mc) : 0.f;
-          s[4 * jj + 2 * h + e] = pr;
-          l_blk += pr;
-        }
-      l_run[h] = l_run[h] * alpha + l_blk;  // this thread's partial row sum (the quad is summed at the end)
-      m_run[h] = m_new;
-#pragma unroll
-      for (int ch = 0; ch < NCH; ++ch)
-#pragma unroll
-        for (int jj = 0; jj < AT_CHUNK / 8; ++jj) o[ch][4 * jj + 2 * h] *= alpha, o[ch][4 * jj + 2 * h + 1] *= alpha;
-    }
-#pragma unroll
-    for (int kk = 0; kk < BKV / 16; ++kk) {
-      pa[kk][0] = pack_bf16(s[8 * kk + 0], s[8 * kk + 1]);
-      pa[kk][1] = pack_bf16(s[8 * kk + 2], s[8 * kk + 3]);
-      pa[kk][2] = pack_bf16(s[8 * kk + 4], s[8 * kk + 5]);
-      pa[kk][3] = pack_bf16(s[8 * kk + 6], s[8 * kk + 7]);
-    }
-    wgmma_fence();
+  };
+  auto issue_pv = [&](int st) {
+    const uint32_t v_addr = kv_base + st * P::STAGE + NCH * P::KV_CHUNK;
 #pragma unroll
     for (int kk = 0; kk < BKV / 16; ++kk)  // B = V: MN-major, 16 keys = 16 rows of 128 B
 #pragma unroll
       for (int ch = 0; ch < NCH; ++ch)
         Wgmma<AT_CHUNK>::rs<1>(o[ch], pa[kk], gmma_desc(v_addr + ch * P::KV_CHUNK + kk * 16 * 128, 8192, 1024), 1u);
     wgmma_commit();
+  };
+  // One key block: S_j = Q K_j^T, its softmax into bf16 P_j fragments, O *= alpha, O += P_j V_j.
+  auto step = [&](auto masked, int j) {
+    const int st = j % NST;
+    mbar_wait(&kv_full[st], (j / NST) & 1);
+    wgmma_fence();
+    issue_s(st);
     wgmma_wait<0>();
+    reg_fence(s);
+    float alpha[2];
+    softmax_block<BKV, decltype(masked)::value>(s, pa, m_run, l_run, alpha, row0, p.nk, p.causal, j * BKV, t4,
+                                                   poly_lane, c);
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int ch = 0; ch < NCH; ++ch)
+#pragma unroll
+        for (int jj = 0; jj < AT_CHUNK / 8; ++jj) o[ch][4 * jj + 2 * h] *= alpha[h], o[ch][4 * jj + 2 * h + 1] *= alpha[h];
+#pragma unroll
+    for (int ch = 0; ch < NCH; ++ch) reg_fence(o[ch]);
+#pragma unroll
+    for (int kk = 0; kk < BKV / 16; ++kk) reg_fence(pa[kk]);
+    wgmma_fence();
+    issue_pv(st);
+    wgmma_wait<0>();
+#pragma unroll
+    for (int ch = 0; ch < NCH; ++ch) reg_fence(o[ch]);
     __syncwarp();
     if (lane == 0) mbar_arrive(&kv_empty[st]);
-  }
+  };
+
+  // blocks [0, n_full) lie below nk and, when causal, end at or before the tile's first query row.  The bound is the
+  // same for the whole CTA (not per warpgroup) so that the compiler sees uniform control flow around the wgmmas.
+  const int full_lim = p.causal ? min(p.nk, q0 + 1) : p.nk;
+  const int n_full = min(nkb, full_lim / BKV);
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < n_full; ++j) step(std::false_type(), j);
+  for (int j = n_full; j < nkb; ++j) step(std::true_type(), j);
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     float l = l_run[h];
     l += __shfl_xor_sync(0xffffffffu, l, 1);
     l += __shfl_xor_sync(0xffffffffu, l, 2);
-    const int row = rq[h];
+    const int row = row0 + 8 * h;
     if (row < p.nq) {
       const float inv = 1.0f / l;
       __nv_bfloat16* out = p.out + (static_cast<size_t>(b) * p.nq + row) * p.ldo + head * D + 2 * t4;

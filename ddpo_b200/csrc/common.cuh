@@ -117,18 +117,14 @@ __device__ __forceinline__ float ex2_poly(float x) {
   return __int_as_float(__float_as_int(p) + ((__float_as_int(r) - 0x4B400000) << 23));
 }
 
-// Which columns of a 32-wide chunk take the polynomial: every DDPO_EXP_POLY_FWD-th one (0 = none).  The split
-// is a fixed function of the element's position, so results stay deterministic and batch invariant.
+// Which score columns of the attention forward take the polynomial: every DDPO_EXP_POLY_FWD-th one (0 = none), column
+// col with col % DDPO_EXP_POLY_FWD == DDPO_EXP_POLY_FWD - 1 (the per-lane select in attention.cu softmax_block).  The
+// split is a fixed function of the element's position, so results stay deterministic and batch invariant.
 // The polynomial costs ~10 issue slots against 1 for MUFU.EX2, so only the forward kernel (fewer other instructions
 // per score) keeps a small share; the backward uses MUFU alone.
 #ifndef DDPO_EXP_POLY_FWD
 #define DDPO_EXP_POLY_FWD 8
 #endif
-template <int PERIOD>
-__device__ __forceinline__ float ex2_sel(int i, float x) {
-  if (PERIOD > 0 && (i % (PERIOD > 0 ? PERIOD : 1)) == PERIOD - 1) return ex2_poly(x);
-  return ex2_mufu(x);
-}
 
 // --------------------------------------------------------------- mbarrier ----
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -212,6 +208,19 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// Pins the registers of a wgmma operand at this point of the instruction order: after a wgmma_wait (the wait names no
+// registers, so the compiler could hoist a use of the accumulators above it), and before a wgmma_fence (so that the
+// instructions defining them are not sunk past it into the wgmma pipeline, which ptxas would serialise).
+template <int N>
+__device__ __forceinline__ void reg_fence(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+template <int N>
+__device__ __forceinline__ void reg_fence(uint32_t (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
 }
 // barrier among `count` threads (a multiple of 32) on hardware barrier `id` (id 0 is __syncthreads)
 __device__ __forceinline__ void named_barrier(int id, int count) {
