@@ -129,6 +129,9 @@ SIGNATURES = {
     "ddpo_pair_stats_u8": (i32, [vp, i32, i32, i32, i32, vp, vp]),
     "ddpo_feature_angles": (i32, [vp, i32, i32, i32, vp, vp]),
     "ddpo_scaled_cosine": (i32, [vp, vp, i32, i32, f32, vp, vp]),
+    "ddpo_lora_merge": (i32, [vp, i32, i32, vp, vp, i32, f32, vp, i32, i32, vp, i32, i32, vp, vp]),
+    "ddpo_lora_grad_workspace_floats": (i64, [i32, i32, i32, i32, i32]),
+    "ddpo_lora_grad": (i32, [vp, i32, vp, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp, i64, vp]),
 }
 
 _lib = None

@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libddpo_b200.so")
 SOURCES = ["abi.cu", "igemm.cu", "wgrad.cu", "attention.cu", "attention_bwd.cu", "norm.cu", "elementwise.cu",
            "backward_ew.cu", "ddim.cu", "rwr.cu", "vae.cu", "text.cu", "vision.cu", "optim.cu",
-           "adafactor.cu", "image_rewards.cu"]
+           "adafactor.cu", "image_rewards.cu", "lora.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

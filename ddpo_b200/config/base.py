@@ -33,6 +33,9 @@ base = {
         # extension (not in the reference): timesteps of one minibatch stacked into one U-Net pass; 1 = the
         # reference's call sequence (ddpo_b200/pipeline/policy_gradient.py)
         "train_macro": 10,
+        # extension: rank (4, 8 or 16) of LoRA adapters on the attention projections, trained with the U-Net frozen;
+        # 0 = full fine-tuning, the reference's only mode
+        "lora_rank": 0,
     },
 }
 

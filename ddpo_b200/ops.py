@@ -741,3 +741,46 @@ def l2norm_rows(x, y):
     m, c = x.shape
     _e = _ev()
     _run("l2norm_rows", lib().ddpo_l2norm_rows(_p(x), _p(y), m, c, _stream()), 0.0, _e)
+
+
+# ------------------------------------------------------------ LoRA adapters -------
+LORA_RANKS = (4, 8, 16)
+
+
+def lora_merge(w, down, up, k, n, rank, fwd=None, ldk=0, row_offset=0, dgrad=None, ld_dst=0, col_offset=0, merged=None,
+               scale=1.0):
+    """bf16(w + scale down @ up) for w fp32 [k, n], down [k, rank], up [rank, n], into the forward operand layout of
+    ``prep_weight`` (``fwd``) and / or the dgrad layout of ``prep_weight_dgrad`` (``dgrad``); ``merged``: the fp32 sum"""
+    _e = _ev()
+    _run("lora_merge", lib().ddpo_lora_merge(_p(w), int(k), int(n), _p(down), _p(up), int(rank), float(scale), _p(fwd),
+                                             int(ldk), int(row_offset), _p(dgrad), int(ld_dst), int(col_offset),
+                                             _p(merged), _stream()), 0.0, _e)
+
+
+_LORA_WS = {}
+_KERNELS_PER_CALL["lora_grad"] = 2
+
+
+def lora_grad(x, dys, downs, ups, d_downs, d_ups, m, k, n, rank, ldx=0, lddy=0, scale=1.0):
+    """For adapters i sharing x bf16 [m, k]: d_ups[i] += scale (x downs[i])^T dys[i] and d_downs[i] += scale x^T
+    (dys[i] ups[i]^T); dys[i] bf16 [m, n] with row pitch ``lddy``.  One launch reads x and every dy once."""
+    g = len(dys)
+    assert 1 <= g <= 3 and len(downs) == len(ups) == len(d_downs) == len(d_ups) == g
+    need = int(lib().ddpo_lora_grad_workspace_floats(int(rank), g, int(m), int(k), int(n)))
+    if need < 0:
+        raise ValueError(f"lora_grad: no tiling for k={k}, n={n}, {g} adapters at rank {rank}")
+    dev = x.device
+    ws = _LORA_WS.get(dev)
+    if ws is None or ws.numel() < need:
+        ws = torch.empty(max(need, 1 << 20), dtype=torch.float32, device=dev)
+        _LORA_WS[dev] = ws
+    arr = lambda ts: (C.c_void_p * g)(*[t.data_ptr() for t in ts])   # noqa: E731
+    for t in list(dys) + [x]:
+        assert t.is_cuda and t.dtype == torch.bfloat16
+    for t in list(downs) + list(ups) + list(d_downs) + list(d_ups):
+        assert t.is_cuda and t.dtype == torch.float32
+    _e = _ev()
+    _run("lora_grad", lib().ddpo_lora_grad(_p(x), int(ldx or k), arr(dys), int(lddy or n), arr(downs), arr(ups),
+                                           arr(d_downs), arr(d_ups), g, int(m), int(k), int(n), int(rank), float(scale),
+                                           _p(ws), ws.numel(), _stream()),
+         float(m) * (k + g * n) * 2, _e, f"M{m} K{k} N{n} G{g} r{rank}" if _e is not None else "")

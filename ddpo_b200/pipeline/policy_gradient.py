@@ -282,6 +282,9 @@ def main(argv=None, models=None, max_epochs=None, save_last=True):
     if args.optimizer not in optimizers:
         raise ValueError(f"optimizer={args.optimizer!r}: must be one of {', '.join(optimizers)}")
     tx = optimizers[args.optimizer]()
+    lora_rank = int(getattr(args, "lora_rank", 0) or 0)
+    if lora_rank:   # adapters on the attention projections, the U-Net frozen; args.seed carries + rank (utils/parser.py):
+        pipeline.unet.enable_lora(lora_rank, seed=args.seed - worker_id)   # every rank builds the same adapters
     state = AccumulatingTrainState(step=0, apply_fn=pipeline.unet, params=params["unet"], tx=tx, n_acc=0)  # :156-164
 
     timer = utils.Timer()
@@ -404,9 +407,10 @@ def main(argv=None, models=None, max_epochs=None, save_last=True):
         t_train = time.time() - t_train0
 
         if (epoch + 1) % args.save_freq == 0 or (epoch == n_epochs - 1 and save_last):                     # :457-464
+            # LoRA mode: the checkpoint holds the merged U-Net (W + D U), so that its readers see a fine-tuned U-Net
+            flat = pipeline.unet.merged_params() if lora_rank else state.params
             utils.save_checkpoint_multiprocess(os.path.join(args.savepath, "checkpoints"),
-                                               utils.params_tree(state.params, cfg), step=epoch, keep=1e6,
-                                               overwrite=True)
+                                               utils.params_tree(flat, cfg), step=epoch, keep=1e6, overwrite=True)
         history.append(dict(epoch=epoch, mean_reward=mean_rewards[-1], std_reward=std_rewards[-1],
                             sample_seconds=t_sample, train_seconds=t_train, infos=epoch_infos,
                             samples=sizes["total_samples_per_epoch"]))

@@ -56,7 +56,8 @@ class AdafactorConfig:
 
 class AccumulatingTrainState:
     """Accumulates gradients over several ``train_step`` calls and applies them when ``do_update``
-    (reference :13-57).  ``params`` / ``grad_acc`` are the U-Net's flat fp32 buffers.  ``tx`` picks the optimizer:
+    (reference :13-57).  ``params`` / ``grad_acc`` are the U-Net's flat fp32 buffers -- or, on a U-Net in LoRA mode
+    (``UNet.enable_lora``), its flat adapter buffers, the U-Net itself staying frozen.  ``tx`` picks the optimizer:
     AdamW keeps ``mu`` (bf16) and ``nu`` (fp32) over the whole buffer; Adafactor keeps only its factored second
     moments, one flat fp32 ``state`` laid out by the host planner (``adafactor_leaves`` names its per-tensor views)."""
 
@@ -65,13 +66,15 @@ class AccumulatingTrainState:
         self.step = int(step)
         self.apply_fn = apply_fn
         apply_fn.enable_training()
-        self.params = apply_fn.params
+        lora = apply_fn.lora_rank > 0
+        self.params = apply_fn.lora_params if lora else apply_fn.params
         self.tx = tx or AdamWConfig()
-        self.grad_acc = apply_fn.grads
+        self.grad_acc = apply_fn.lora_grads if lora else apply_fn.grads
+        self._table = apply_fn.lora_table if lora else apply_fn.table
         self.n_acc = int(n_acc)
         dev = self.params.device
         if isinstance(self.tx, AdafactorConfig):
-            self._plan = ops.adafactor_plan(list(apply_fn.table.values()), self.params.numel(),
+            self._plan = ops.adafactor_plan(list(self._table.values()), self.params.numel(),
                                             self.tx.min_dim_size_to_factor)
             self._af_ws = torch.empty(self._plan.workspace_floats, dtype=torch.float32, device=dev)
             if opt_state is None:
@@ -91,7 +94,7 @@ class AccumulatingTrainState:
     def adafactor_leaves(self):
         """Adafactor only: parameter name -> {"v_row", "v_col"} or {"v"} views of the state, shaped as optax's."""
         views = self._plan.state_views(self.opt_state["state"])
-        return dict(zip(self.apply_fn.table, views))
+        return dict(zip(self._table, views))
 
     def apply_gradients(self, *, grads=None, do_update: bool, n_micro: int = 1, **kwargs):
         """``grads`` is accepted for signature parity; the backward pass has already added this step's

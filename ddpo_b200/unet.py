@@ -24,7 +24,7 @@ import torch
 
 from . import ops
 from .ops import ATTENTION_HEAD_DIMS
-from .unet_spec import UNetConfig, param_offsets
+from .unet_spec import UNetConfig, init_lora_params, lora_manifest, lora_offsets, param_offsets
 
 BF16 = torch.bfloat16
 F32 = torch.float32
@@ -112,6 +112,11 @@ class UNet:
         self._temb_names = [n[: -len("/time_emb_proj/kernel")] for n in self.table if n.endswith("/time_emb_proj/kernel")]
         self._temb_tables: Dict[int, tuple] = {}
         self._tproj_views: Optional[Dict[str, torch.Tensor]] = None
+        # LoRA mode (enable_lora): the U-Net is frozen and only the adapters of the attention projections train
+        self.lora_rank = 0
+        self.lora_params: Optional[torch.Tensor] = None   # flat fp32 adapters (lora_table layout)
+        self.lora_grads: Optional[torch.Tensor] = None
+        self.lora_table: Dict[str, tuple] = {}
         self.refresh_weights()
 
     # ------------------------------------------------------------------ params ----
@@ -132,13 +137,31 @@ class UNet:
             out.append((base, shape))
         return out
 
+    def _lora_views(self, base):
+        """(down, up) adapter views of an adapted layer, or None"""
+        if base + "/lora_down" not in self.lora_table:
+            return None
+        return self.lp(base + "/lora_down"), self.lp(base + "/lora_up")
+
     def refresh_weights(self):
-        """fp32 Flax params -> bf16 [N, K] GEMM operands (run after every optimizer step)."""
+        """fp32 Flax params -> bf16 [N, K] GEMM operands (run after every optimizer step).  In LoRA mode the adapted
+        layers' operands are bf16(W + D U) (ops.lora_merge), and once built only those are re-merged: nothing else
+        changes."""
+        adapted_only = self.lora_rank > 0 and getattr(self, "_frozen_ready", False)
         for base, shape in self._layers:
             leaf = base.rsplit("/", 1)[1]
+            lora = self._lora_views(base)
+            if adapted_only and lora is None:
+                continue
             src = self.p(base + "/kernel")
             k = int(np.prod(shape[:-1]))
             n = int(shape[-1])
+
+            def prep(dst, row_offset=0):
+                if lora is None:
+                    ops.prep_weight(src, dst, k, n, row_offset=row_offset)
+                else:
+                    ops.lora_merge(src, lora[0], lora[1], k, n, self.lora_rank, fwd=dst, ldk=k, row_offset=row_offset)
             if leaf in ("to_q", "to_k", "to_v"):
                 attn = base.rsplit("/", 1)[0]
                 is_self = attn.endswith("attn1")
@@ -146,17 +169,22 @@ class UNet:
                     key = attn + "/qkv"
                     if key not in self.w:
                         self.w[key] = torch.empty(3 * n, k, dtype=BF16, device=self.device)
-                    ops.prep_weight(src, self.w[key], k, n, row_offset={"to_q": 0, "to_k": n, "to_v": 2 * n}[leaf])
+                    prep(self.w[key], row_offset={"to_q": 0, "to_k": n, "to_v": 2 * n}[leaf])
                 elif leaf == "to_q":
                     key = attn + "/q"
                     if key not in self.w:
                         self.w[key] = torch.empty(n, k, dtype=BF16, device=self.device)
-                    ops.prep_weight(src, self.w[key], k, n)
+                    prep(self.w[key])
                 else:
                     key = attn + "/kv"
                     if key not in self.w:
                         self.w[key] = torch.empty(2 * n, k, dtype=BF16, device=self.device)
-                    ops.prep_weight(src, self.w[key], k, n, row_offset=0 if leaf == "to_k" else n)
+                    prep(self.w[key], row_offset=0 if leaf == "to_k" else n)
+                continue
+            if lora is not None:                   # to_out_0
+                if base not in self.w:
+                    self.w[base] = torch.empty(n, k, dtype=BF16, device=self.device)
+                prep(self.w[base])
                 continue
             if base not in self.w:
                 self.w[base] = torch.empty(n, k, dtype=BF16, device=self.device)
@@ -168,36 +196,98 @@ class UNet:
             else:
                 ops.prep_weight(src, self.w[base], k, n)
         if self.train_mode:
-            self._refresh_dgrad_weights()
+            self._refresh_dgrad_weights(adapted_only)
+        if self.lora_rank > 0 and self.train_mode:
+            self._frozen_ready = True
 
     def enable_training(self):
-        """Allocates the gradient accumulator and the dgrad-layout bf16 weights."""
-        if self.grads is None:
+        """Allocates the gradient accumulator (full fine-tuning only: in LoRA mode the adapters' gradient buffer is
+        ``lora_grads``) and the dgrad-layout bf16 weights."""
+        if self.grads is None and self.lora_rank == 0:
             self.grads = torch.zeros_like(self.params)
         self.train_mode = True
-        self._refresh_dgrad_weights()
+        self._refresh_dgrad_weights(False)
+        if self.lora_rank > 0:
+            self._frozen_ready = True
 
-    def _refresh_dgrad_weights(self):
+    def enable_lora(self, rank: int, seed: int = 0):
+        """LoRA mode: rank-``rank`` adapters (diffusers' LoRALinearLayer, scale 1) on to_q / to_k / to_v / to_out_0 of
+        both attentions of every transformer block, the rest of the U-Net frozen.  Builds the adapter table, the flat
+        fp32 adapters (down ~ N(0, 1/rank^2), up = 0, from a seeded host generator) and their gradient buffer; the
+        U-Net's own gradient buffer is never allocated.  Call before ``enable_training``."""
+        assert self.grads is None, "enable_lora() on a U-Net that already trains all of its parameters"
+        self.lora_table, total = lora_offsets(self.cfg, rank)
+        self.lora_rank = int(rank)
+        self.lora_params = init_lora_params(self.cfg, rank, seed).to(self.device)
+        self.lora_grads = torch.zeros(total, dtype=F32, device=self.device)
+        # where the kernels that always produce a parameter gradient (norm backwards, conv_out) put it in LoRA mode;
+        # kernel / scale and bias get separate halves
+        self._discard = torch.zeros(2, 16384, dtype=F32, device=self.device)
+        self._frozen_ready = False
+        self.refresh_weights()
+        return self
+
+    def lp(self, name):
+        off, shape = self.lora_table[name]
+        return self.lora_params[off:off + int(np.prod(shape))].view(*shape)
+
+    def lg(self, name):
+        off, shape = self.lora_table[name]
+        return self.lora_grads[off:off + int(np.prod(shape))].view(*shape)
+
+    def merged_params(self) -> torch.Tensor:
+        """The flat fp32 parameters, in host memory, with every adapted kernel replaced by W + D U (the U-Net the
+        adapters define; what a checkpoint of a LoRA run holds).  Without adapters: a host copy of ``params``.  The
+        kernels are merged one at a time through a small device buffer, so that saving a checkpoint does not hold a
+        second copy of the U-Net on the device."""
+        out = self.params.cpu().clone() if self.params.is_cuda else self.params.clone()
+        scratch = None
+        for _, _, kernel in lora_manifest(self.cfg, self.lora_rank)[::2] if self.lora_rank else ():
+            base = kernel[: -len("/kernel")]
+            off, (k, n) = self.table[kernel]
+            if scratch is None or scratch.numel() < k * n:
+                scratch = torch.empty(k * n, dtype=F32, device=self.device)
+            down, up = self._lora_views(base)
+            merged = scratch[:k * n].view(k, n)
+            ops.lora_merge(self.p(base + "/kernel"), down, up, k, n, self.lora_rank, merged=merged)
+            out[off:off + k * n].copy_(merged.reshape(-1))
+        return out
+
+    def _refresh_dgrad_weights(self, adapted_only=False):
         for base, shape in self._layers:
             leaf = base.rsplit("/", 1)[1]
             if leaf in ("to_k", "to_v") and "/attn2/" in base:
                 continue  # the text context receives no gradient
+            lora = self._lora_views(base)
+            if adapted_only and lora is None:
+                continue
             cin, n = int(shape[-2]), int(shape[-1])
+
+            def prep(dst, ld_dst=0, col_offset=0):
+                if lora is None:
+                    ops.prep_weight_dgrad(self.p(base + "/kernel"), dst, 1, cin, n, ld_dst=ld_dst, col_offset=col_offset)
+                else:
+                    ops.lora_merge(self.p(base + "/kernel"), lora[0], lora[1], cin, n, self.lora_rank, dgrad=dst,
+                                   ld_dst=ld_dst, col_offset=col_offset)
             if leaf in ("to_q", "to_k", "to_v") and "/attn1/" in base:
                 # the input gradient of self-attention is ONE GEMM over K = 3C: d_ln = [dq | dk | dv] [Wq | Wk | Wv]^T
                 key = base.rsplit("/", 1)[0] + "/qkv"
                 if key not in self.wd:
                     self.wd[key] = torch.empty(cin, 3 * n, dtype=BF16, device=self.device)
-                ops.prep_weight_dgrad(self.p(base + "/kernel"), self.wd[key], 1, cin, n, ld_dst=3 * n,
-                                      col_offset={"to_q": 0, "to_k": n, "to_v": 2 * n}[leaf])
+                prep(self.wd[key], ld_dst=3 * n, col_offset={"to_q": 0, "to_k": n, "to_v": 2 * n}[leaf])
                 continue
             taps = int(np.prod(shape[:-2])) if len(shape) == 4 else 1
             if base not in self.wd:
                 self.wd[base] = torch.empty(cin, taps * n, dtype=BF16, device=self.device)
-            ops.prep_weight_dgrad(self.p(base + "/kernel"), self.wd[base], taps, cin, n)
+            if lora is not None:
+                prep(self.wd[base])
+            else:
+                ops.prep_weight_dgrad(self.p(base + "/kernel"), self.wd[base], taps, cin, n)
 
     def g(self, name):
         off, shape = self.table[name]
+        if self.lora_rank > 0:   # frozen: a scratch destination for the kernels that always write a parameter gradient
+            return self._discard[int(name.endswith("/bias")), :int(np.prod(shape))].view(*shape)
         return self.grads[off:off + int(np.prod(shape))].view(*shape)
 
     # ----------------------------------------------------------------- context ----
@@ -481,8 +571,12 @@ class UNet:
     # ---------------------------------------------------------------- backward ----
     def backward(self, tape: list, d_eps: torch.Tensor):
         """Back-propagates d(loss)/d(eps) [B,4,H,W] through the taped forward; parameter gradients are
-        ACCUMULATED into ``self.grads`` (AccumulatingTrainState semantics).  Releases the tape's buffers."""
-        assert self.train_mode and self.grads is not None
+        ACCUMULATED into ``self.grads`` (AccumulatingTrainState semantics).  Releases the tape's buffers.
+        In LoRA mode every data gradient is computed exactly as in full fine-tuning, no base-parameter gradient is
+        formed (no weight-gradient GEMMs, bias sums or time-embedding chain), and the adapter gradients are
+        accumulated into ``self.lora_grads`` (ops.lora_grad)."""
+        assert self.train_mode and (self.grads is not None or self.lora_rank > 0)
+        full = self.lora_rank == 0
         A = self.arena
         grads: Dict[int, torch.Tensor] = {}
 
@@ -503,7 +597,9 @@ class UNet:
 
         def bias_grad_and_cast(dy, m, n, bias_names):
             dyb = A.alloc((m, n), BF16)
-            if len(bias_names) == 1:
+            if not full:                       # frozen biases: the bf16 copy only
+                ops.cast_bf16(dy, dyb)
+            elif len(bias_names) == 1:
                 ops.colsum_cast(dy, m, n, y_bf16=dyb, out=self.g(bias_names[0]).view(1, n), accumulate=True)
             else:
                 tmp = A.alloc((1, n), F32)
@@ -531,7 +627,9 @@ class UNet:
                 m2 = b * 4 * h * w
                 dy = grads.pop(id(r["out"]))
                 dyb = bias_grad_and_cast(dy, m2, c, [name + "/conv/bias"])
-                ops.wgrad(dy=dyb, n=c, x0=r["up"], c0=c, conv=(b, 2 * h, 2 * w), taps=9, dw=self.g(name + "/conv/kernel"))
+                if full:
+                    ops.wgrad(dy=dyb, n=c, x0=r["up"], c0=c, conv=(b, 2 * h, 2 * w), taps=9,
+                              dw=self.g(name + "/conv/kernel"))
                 d_up = A.alloc((m2, c), F32)
                 ops.igemm(a0=dyb, wt=self.wd[name + "/conv"], n=c, c0=c, conv=(b, 2 * h, 2 * w), taps=9, out_f32=d_up)
                 if id(r["x"]) in grads:
@@ -547,8 +645,9 @@ class UNet:
                 mo = b * (h // 2) * (w // 2)
                 dy = grads.pop(id(r["out"]))
                 dyb = bias_grad_and_cast(dy, mo, c, [name + "/conv/bias"])
-                ops.wgrad(dy=dyb, n=c, x0=r["xb"], c0=c, conv=(b, h // 2, w // 2), taps=9, stride=2,
-                          dw=self.g(name + "/conv/kernel"))
+                if full:
+                    ops.wgrad(dy=dyb, n=c, x0=r["xb"], c0=c, conv=(b, h // 2, w // 2), taps=9, stride=2,
+                              dw=self.g(name + "/conv/kernel"))
                 dil = A.alloc((b * h * w, c), BF16)
                 ops.dilate2x_bf16(dy, dil, b, h // 2, w // 2, c)
                 if id(r["x"]) in grads:
@@ -570,8 +669,9 @@ class UNet:
                 te = self.cfg.time_embed_dim
                 x = r.get("x")
                 dx = grads.pop(id(x))
-                ops.colsum_cast(dx, b * H * W, c0, out=self.g("conv_in/bias").view(1, c0), accumulate=True)
-                ops.conv_in_wgrad(r["latents"], dx, self.g("conv_in/kernel"), b, self.cfg.in_channels, H, W, c0)
+                if full:
+                    ops.colsum_cast(dx, b * H * W, c0, out=self.g("conv_in/bias").view(1, c0), accumulate=True)
+                    ops.conv_in_wgrad(r["latents"], dx, self.g("conv_in/kernel"), b, self.cfg.in_channels, H, W, c0)
                 A.release(dx)
                 A.release(x)
                 d_temb = temb_state["d"]
@@ -601,9 +701,11 @@ class UNet:
         dy = grads.pop(id(r["out"]))
         if getattr(self, "_dbg", None) is not None:
             self._dbg[name] = dy.clone()
+        full = self.lora_rank == 0
         names = [name + "/conv2/bias"] + ([name + "/conv_shortcut/bias"] if r["has_sc"] else [])
         dyb = bias_grad_and_cast(dy, m, cout, names)
-        ops.wgrad(dy=dyb, n=cout, x0=r["a2"], c0=cout, conv=(b, h, w), taps=9, dw=self.g(name + "/conv2/kernel"))
+        if full:
+            ops.wgrad(dy=dyb, n=cout, x0=r["a2"], c0=cout, conv=(b, h, w), taps=9, dw=self.g(name + "/conv2/kernel"))
         # gradients that go straight from a dgrad GEMM into a norm's backward travel as bf16 (half the bytes on both sides;
         # the forward value they belong to was itself a bf16 GEMM operand)
         d_a2 = A.alloc((m, cout), BF16)
@@ -614,26 +716,31 @@ class UNet:
         A.release(d_a2)
         # h = conv1(a) + bias1 + time_emb_proj(silu(temb))[b]
         d_hb = A.alloc((m, cout), BF16)
-        d_tproj = A.alloc((b, cout), F32)
-        ops.colsum_cast(d_h, m, cout, y_bf16=d_hb, out=d_tproj, rows_per_group=hw, accumulate=False)
-        A.release(d_h)
-        ops.colsum_cast(d_tproj, b, cout, out=self.g(name + "/conv1/bias").view(1, cout), accumulate=True)
-        first = temb_state["d"] is None
-        if first:
-            temb_state["d"] = A.alloc((b, te), F32)
-        dpre = A.alloc((b, cout), F32)
-        ops.dense_small_bwd(self._temb_act, self.p(name + "/time_emb_proj/kernel"), None, d_tproj, dpre,
-                            self.g(name + "/time_emb_proj/kernel"), self.g(name + "/time_emb_proj/bias"),
-                            temb_state["d"], b, te, cout, dx_accumulate=not first)
-        A.release(dpre)
-        A.release(d_tproj)
-        ops.wgrad(dy=d_hb, n=cout, x0=r["a"], c0=cin, conv=(b, h, w), taps=9, dw=self.g(name + "/conv1/kernel"))
+        if full:
+            d_tproj = A.alloc((b, cout), F32)
+            ops.colsum_cast(d_h, m, cout, y_bf16=d_hb, out=d_tproj, rows_per_group=hw, accumulate=False)
+            A.release(d_h)
+            ops.colsum_cast(d_tproj, b, cout, out=self.g(name + "/conv1/bias").view(1, cout), accumulate=True)
+            first = temb_state["d"] is None
+            if first:
+                temb_state["d"] = A.alloc((b, te), F32)
+            dpre = A.alloc((b, cout), F32)
+            ops.dense_small_bwd(self._temb_act, self.p(name + "/time_emb_proj/kernel"), None, d_tproj, dpre,
+                                self.g(name + "/time_emb_proj/kernel"), self.g(name + "/time_emb_proj/bias"),
+                                temb_state["d"], b, te, cout, dx_accumulate=not first)
+            A.release(dpre)
+            A.release(d_tproj)
+            ops.wgrad(dy=d_hb, n=cout, x0=r["a"], c0=cin, conv=(b, h, w), taps=9, dw=self.g(name + "/conv1/kernel"))
+        else:                                  # frozen time embedding: no d_tproj, no chain into temb
+            ops.cast_bf16(d_h, d_hb)
+            A.release(d_h)
         d_a = A.alloc((m, cin), BF16)
         ops.igemm(a0=d_hb, wt=self.wd[name + "/conv1"], n=cin, c0=cout, conv=(b, h, w), taps=9, out_bf16=d_a)
         A.release(d_hb)
         if r["has_sc"]:
-            ops.wgrad(dy=dyb, n=cout, x0=r["raw"], c0=cin, conv=(b, h, w), taps=1,
-                      dw=self.g(name + "/conv_shortcut/kernel"))
+            if full:
+                ops.wgrad(dy=dyb, n=cout, x0=r["raw"], c0=cin, conv=(b, h, w), taps=1,
+                          dw=self.g(name + "/conv_shortcut/kernel"))
             dcat = A.alloc((m, cin), F32)
             ops.igemm(a0=dyb, wt=self.wd[name + "/conv_shortcut"], n=cin, c0=cout, conv=(b, h, w), taps=1, out_f32=dcat)
             ops.groupnorm_bwd(r["x0"], self.p(name + "/norm1/scale"), self.p(name + "/norm1/bias"), r["gws"], b, hw, c0,
@@ -670,12 +777,21 @@ class UNet:
         bl = name + "/transformer_blocks_0"
         L = self.ctx_len
         dctx = self.cfg.cross_attention_dim
+        full = self.lora_rank == 0
+
+        def lora_grad(x, dys, ld, projs, attn, mm, k):
+            """adapter gradients of the projections ``projs`` of ``attn``, which share the input x [mm, k]"""
+            bases = [f"{bl}/{attn}/{p}" for p in projs]
+            ops.lora_grad(x, dys, [self.lp(b_ + "/lora_down") for b_ in bases], [self.lp(b_ + "/lora_up") for b_ in bases],
+                          [self.lg(b_ + "/lora_down") for b_ in bases], [self.lg(b_ + "/lora_up") for b_ in bases],
+                          mm, k, c, self.lora_rank, lddy=ld)
         dy = grads.pop(id(t["out"]))
         if getattr(self, "_dbg", None) is not None:
             self._dbg[name] = dy.clone()
         # out = proj_out(h3b) + x
         dyb = bias_grad_and_cast(dy, m, c, [name + "/proj_out/bias"])
-        ops.wgrad(dy=dyb, n=c, x0=t["h3b"], c0=c, m=m, dw=self.g(name + "/proj_out/kernel").view(c, c))
+        if full:
+            ops.wgrad(dy=dyb, n=c, x0=t["h3b"], c0=c, m=m, dw=self.g(name + "/proj_out/kernel").view(c, c))
         d_h = A.alloc((m, c), F32)   # running gradient of the transformer-internal residual stream
         ops.igemm(a0=dyb, wt=self.wd[name + "/proj_out"], n=c, c0=c, m=m, out_f32=d_h)
         A.release(dyb)
@@ -684,15 +800,17 @@ class UNet:
             A.release(dy)
         # h3 = ff2(ff) + h2
         d3b = bias_grad_and_cast(d_h, m, c, [bl + "/ff/net_2/bias"])
-        ops.wgrad(dy=d3b, n=c, x0=t["ff"], c0=4 * c, m=m, dw=self.g(bl + "/ff/net_2/kernel"))
+        if full:
+            ops.wgrad(dy=d3b, n=c, x0=t["ff"], c0=4 * c, m=m, dw=self.g(bl + "/ff/net_2/kernel"))
         d_ff = A.alloc((m, 4 * c), BF16)
         ops.igemm(a0=d3b, wt=self.wd[bl + "/ff/net_2"], n=4 * c, c0=c, m=m, out_bf16=d_ff)
         A.release(d3b)
         d_pre = A.alloc((m, 8 * c), BF16)
         ops.geglu_bwd(t["ffpre"], d_ff, d_pre, m, 8 * c, 256)
         A.release(d_ff)
-        ops.colsum_bf16(d_pre, m, 8 * c, self.g(bl + "/ff/net_0/proj/bias").view(1, 8 * c), accumulate=True)
-        ops.wgrad(dy=d_pre, n=8 * c, x0=t["ln3"], c0=c, m=m, dw=self.g(bl + "/ff/net_0/proj/kernel"))
+        if full:
+            ops.colsum_bf16(d_pre, m, 8 * c, self.g(bl + "/ff/net_0/proj/bias").view(1, 8 * c), accumulate=True)
+            ops.wgrad(dy=d_pre, n=8 * c, x0=t["ln3"], c0=c, m=m, dw=self.g(bl + "/ff/net_0/proj/kernel"))
         d_ln = A.alloc((m, c), BF16)   # dgrad GEMM -> norm backward: bf16 (see _resnet_bwd)
         ops.igemm(a0=d_pre, wt=self.wd[bl + "/ff/net_0/proj"], n=c, c0=8 * c, m=m, out_bf16=d_ln)
         A.release(d_pre)
@@ -701,7 +819,10 @@ class UNet:
                           self.g(bl + "/norm3/bias"), lws, m, c, accumulate=True)
         # h2 = out2(ao2) + h1   (cross attention)
         d2b = bias_grad_and_cast(d_h, m, c, [bl + "/attn2/to_out_0/bias"])
-        ops.wgrad(dy=d2b, n=c, x0=t["ao2"], c0=c, m=m, dw=self.g(bl + "/attn2/to_out_0/kernel"))
+        if full:
+            ops.wgrad(dy=d2b, n=c, x0=t["ao2"], c0=c, m=m, dw=self.g(bl + "/attn2/to_out_0/kernel"))
+        else:
+            lora_grad(t["ao2"], [d2b], c, ["to_out_0"], "attn2", m, c)
         d_ao = A.alloc((m, c), BF16)
         ops.igemm(a0=d2b, wt=self.wd[bl + "/attn2/to_out_0"], n=c, c0=c, m=m, out_bf16=d_ao)
         A.release(d2b)
@@ -711,9 +832,14 @@ class UNet:
         delta = A.alloc((b, heads, hw), F32)
         ops.attention_bwd(t["q2"], kv, kv[:, c:], t["ao2"], d_ao, t["lse2"], delta, dq2, dkv, dkv[:, c:], b, heads, hw, L,
                           c, 2 * c, 2 * c, c, c, c, 2 * c, 2 * c, **_head_dim_kw(c, heads))
-        ops.wgrad(dy=dq2, n=c, x0=t["ln2"], c0=c, m=m, dw=self.g(bl + "/attn2/to_q/kernel"))
-        ops.wgrad(dy=dkv, ldy=2 * c, n=c, x0=self._ctx_bf, c0=dctx, m=b * L, dw=self.g(bl + "/attn2/to_k/kernel"))
-        ops.wgrad(dy=dkv[:, c:], ldy=2 * c, n=c, x0=self._ctx_bf, c0=dctx, m=b * L, dw=self.g(bl + "/attn2/to_v/kernel"))
+        if full:
+            ops.wgrad(dy=dq2, n=c, x0=t["ln2"], c0=c, m=m, dw=self.g(bl + "/attn2/to_q/kernel"))
+            ops.wgrad(dy=dkv, ldy=2 * c, n=c, x0=self._ctx_bf, c0=dctx, m=b * L, dw=self.g(bl + "/attn2/to_k/kernel"))
+            ops.wgrad(dy=dkv[:, c:], ldy=2 * c, n=c, x0=self._ctx_bf, c0=dctx, m=b * L,
+                      dw=self.g(bl + "/attn2/to_v/kernel"))
+        else:
+            lora_grad(t["ln2"], [dq2], c, ["to_q"], "attn2", m, c)
+            lora_grad(self._ctx_bf, [dkv, dkv[:, c:]], 2 * c, ["to_k", "to_v"], "attn2", b * L, dctx)
         ops.igemm(a0=dq2, wt=self.wd[bl + "/attn2/to_q"], n=c, c0=c, m=m, out_bf16=d_ln)
         ops.layernorm_bwd(t["h1"], self.p(bl + "/norm2/scale"), t["st2"], d_ln, d_h, self.g(bl + "/norm2/scale"),
                           self.g(bl + "/norm2/bias"), lws, m, c, accumulate=True)
@@ -721,7 +847,10 @@ class UNet:
         A.release(dkv)
         # h1 = out1(ao1) + h0   (self attention)
         d1b = bias_grad_and_cast(d_h, m, c, [bl + "/attn1/to_out_0/bias"])
-        ops.wgrad(dy=d1b, n=c, x0=t["ao1"], c0=c, m=m, dw=self.g(bl + "/attn1/to_out_0/kernel"))
+        if full:
+            ops.wgrad(dy=d1b, n=c, x0=t["ao1"], c0=c, m=m, dw=self.g(bl + "/attn1/to_out_0/kernel"))
+        else:
+            lora_grad(t["ao1"], [d1b], c, ["to_out_0"], "attn1", m, c)
         ops.igemm(a0=d1b, wt=self.wd[bl + "/attn1/to_out_0"], n=c, c0=c, m=m, out_bf16=d_ao)
         A.release(d1b)
         qkv = t["qkv"]
@@ -729,8 +858,12 @@ class UNet:
         ops.attention_bwd(qkv, qkv[:, c:], qkv[:, 2 * c:], t["ao1"], d_ao, t["lse1"], delta, dqkv, dqkv[:, c:],
                           dqkv[:, 2 * c:], b, heads, hw, hw, 3 * c, 3 * c, 3 * c, c, c, 3 * c, 3 * c, 3 * c,
                           **_head_dim_kw(c, heads))
-        for i, nm in enumerate(("to_q", "to_k", "to_v")):
-            ops.wgrad(dy=dqkv[:, i * c:], ldy=3 * c, n=c, x0=t["ln1"], c0=c, m=m, dw=self.g(f"{bl}/attn1/{nm}/kernel"))
+        if full:
+            for i, nm in enumerate(("to_q", "to_k", "to_v")):
+                ops.wgrad(dy=dqkv[:, i * c:], ldy=3 * c, n=c, x0=t["ln1"], c0=c, m=m,
+                          dw=self.g(f"{bl}/attn1/{nm}/kernel"))
+        else:
+            lora_grad(t["ln1"], [dqkv, dqkv[:, c:], dqkv[:, 2 * c:]], 3 * c, ["to_q", "to_k", "to_v"], "attn1", m, c)
         ops.igemm(a0=dqkv, c0=3 * c, wt=self.wd[bl + "/attn1/qkv"], n=c, m=m, out_bf16=d_ln)   # one GEMM over K = 3C
         ops.layernorm_bwd(t["h0"], self.p(bl + "/norm1/scale"), t["st1"], d_ln, d_h, self.g(bl + "/norm1/scale"),
                           self.g(bl + "/norm1/bias"), lws, m, c, accumulate=True)
@@ -738,7 +871,8 @@ class UNet:
             A.release(z)
         # h0 = proj_in(g)
         d0b = bias_grad_and_cast(d_h, m, c, [name + "/proj_in/bias"])
-        ops.wgrad(dy=d0b, n=c, x0=t["g"], c0=c, m=m, dw=self.g(name + "/proj_in/kernel").view(c, c))
+        if full:
+            ops.wgrad(dy=d0b, n=c, x0=t["g"], c0=c, m=m, dw=self.g(name + "/proj_in/kernel").view(c, c))
         ops.igemm(a0=d0b, wt=self.wd[name + "/proj_in"], n=c, c0=c, m=m, out_bf16=d_ln)
         A.release(d0b)
         A.release(d_h)

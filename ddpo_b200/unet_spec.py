@@ -155,3 +155,47 @@ def init_flat_params(cfg: UNetConfig, seed: int = 0) -> torch.Tensor:
 def views(flat: torch.Tensor, cfg: UNetConfig) -> Dict[str, torch.Tensor]:
     table, _ = param_offsets(cfg)
     return {k: flat[o:o + int(np.prod(s))].view(*s) for k, (o, s) in table.items()}
+
+
+# ------------------------------------------------------------------ LoRA adapters ----
+LORA_RANKS = (4, 8, 16)
+LORA_PROJECTIONS = ("to_q", "to_k", "to_v", "to_out_0")
+
+
+def lora_manifest(cfg: UNetConfig, rank: int) -> List[Tuple[str, Tuple[int, ...], str]]:
+    """(adapter name, shape, adapted kernel) of diffusers' LoRALinearLayer on the four projections of attn1 and attn2 in
+    every transformer block: ``<attention>/<proj>/lora_down`` [in, rank] (down.weight^T) and ``.../lora_up`` [rank, out]
+    (up.weight^T), in the U-Net's parameter order."""
+    if rank not in LORA_RANKS:
+        raise ValueError(f"lora_rank={rank!r}: must be one of {', '.join(map(str, LORA_RANKS))}")
+    out = []
+    for name, shape in param_manifest(cfg):
+        parts = name.split("/")
+        if len(parts) >= 3 and parts[-3] in ("attn1", "attn2") and parts[-2] in LORA_PROJECTIONS and parts[-1] == "kernel":
+            base = name[: -len("/kernel")]
+            k, n = shape
+            out += [(base + "/lora_down", (k, rank), name), (base + "/lora_up", (rank, n), name)]
+    return out
+
+
+def lora_offsets(cfg: UNetConfig, rank: int, align: int = 64) -> Tuple[Dict[str, Tuple[int, Tuple[int, ...]]], int]:
+    """adapter name -> (offset in floats, shape) in the flat fp32 adapter buffer; every tensor starts 256-byte aligned"""
+    off = 0
+    table = {}
+    for name, shape, _ in lora_manifest(cfg, rank):
+        table[name] = (off, shape)
+        off += (int(np.prod(shape)) + align - 1) // align * align
+    return table, off
+
+
+def init_lora_params(cfg: UNetConfig, rank: int, seed: int = 0) -> torch.Tensor:
+    """diffusers' LoRALinearLayer initialisation: down ~ N(0, (1/rank)^2), up = 0.  Drawn on the host from a seeded
+    generator, so that every data-parallel rank builds the same adapters."""
+    table, total = lora_offsets(cfg, rank)
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    flat = torch.zeros(total, dtype=torch.float32)
+    for name, (off, shape) in table.items():
+        if name.endswith("/lora_down"):
+            n = int(np.prod(shape))
+            flat[off:off + n] = torch.randn(n, generator=g) * (1.0 / rank)
+    return flat

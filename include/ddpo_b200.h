@@ -397,6 +397,26 @@ int ddpo_feature_angles(const float* feats, int variants, int n, int dim, float*
 /* out[i] = exp(logit_scale) * cos(img[i], txt[i]) for fp32 [n, dim] rows, in double */
 int ddpo_scaled_cosine(const float* img, const float* txt, int n, int dim, float logit_scale, float* out, void* stream);
 
+/* ------------------------------------------------------------------ low-rank adapters (LoRA) --------
+ * diffusers' LoRALinearLayer in the Flax layout: y = x W + b + scale (x D) U with W fp32 [k, n], D fp32 [k, rank]
+ * (down.weight^T) and U fp32 [rank, n] (up.weight^T).
+ * lora_merge: bf16(W + scale D U), the rank-sum in fp32 and one rounding, into the forward operand layout of
+ * ddpo_prep_weight (fwd_bf16 [.., ldk], row n + row_offset) and / or the dgrad layout of ddpo_prep_weight_dgrad with
+ * taps = 1 (dgrad_bf16 [k, ld_dst], column col_offset + n) and / or the fp32 sum itself (merged_f32 [k, n]); any
+ * output may be NULL.  ldk <= 0: k, ld_dst <= 0: n.
+ * lora_grad: for g <= 3 adapters that share x bf16 [m, k] (row pitch ldx), with dy[i] bf16 [m, n] (row pitch lddy),
+ * down[i] / up[i] fp32 as above:  d_up[i] += scale (x down[i])^T dy[i],  d_down[i] += scale x^T (dy[i] up[i]^T).
+ * dy, down, up, d_down, d_up are host arrays of g device pointers.  rank is 4, 8 or 16; ldx, lddy multiples of 8 and
+ * x / dy 16-byte aligned.  Deterministic (fixed-order two-stage reduction over m); the workspace (fp32, at least
+ * ddpo_lora_grad_workspace_floats, which is -1 for an unsupported shape) holds one partial per CTA cluster. */
+int ddpo_lora_merge(const float* w, int k, int n, const float* down, const float* up, int rank, float scale,
+                    void* fwd_bf16, int ldk, int row_offset, void* dgrad_bf16, int ld_dst, int col_offset,
+                    float* merged_f32, void* stream);
+int64_t ddpo_lora_grad_workspace_floats(int rank, int g, int m, int k, int n);
+int ddpo_lora_grad(const void* x, int ldx, const void* const* dy, int lddy, const float* const* down,
+                   const float* const* up, float* const* d_down, float* const* d_up, int g, int m, int k, int n,
+                   int rank, float scale, float* workspace, int64_t workspace_floats, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
