@@ -1,7 +1,8 @@
-"""The U-Net forward's kernel launches, recorded without a GPU: ``UNet.prepare_context`` and ``UNet.forward`` run on the
-``meta`` device with ``ddpo_b200.unet.ops`` swapped for a recorder, so every launch's arguments (scalars, and the shape,
-dtype, strides and storage offset of every tensor) are listed exactly as unet.py makes them.  test_forward_layers.py
-replays each distinct configuration on the CUDA library against float64.
+"""The U-Net forward's and the VAE's kernel launches, recorded without a GPU: ``UNet.prepare_context`` and
+``UNet.forward``, ``VAEDecoder.decode`` and ``VAEEncoder.encode`` run on the ``meta`` device with the model module's
+``ops`` swapped for a recorder, so every launch's arguments (scalars, and the shape, dtype, strides and storage offset
+of every tensor) are listed exactly as unet.py / vae.py make them.  test_forward_layers.py and test_vae_layers.py replay
+each distinct configuration on the CUDA library against float64.
 
 A launch's *signature* is its op name and its arguments with every tensor reduced to (shape, dtype, strides, buffer,
 offset): ``buffer`` numbers the distinct storages of the call in order of first use ("P" for the flat parameter buffer,
@@ -17,11 +18,18 @@ import torch
 from ddpo_b200 import ops as real_ops
 from ddpo_b200 import unet as unet_mod
 from ddpo_b200 import unet_spec
+from ddpo_b200 import vae as vae_mod
 
 # (name, config, batch, taped): sampling runs the U-Net at batch 2 x 8 (CFG), the PPO train pass at 40 with a tape
 RUNS = [("sd2", unet_spec.SD2_BASE, 16, False), ("sd2", unet_spec.SD2_BASE, 40, True),
         ("sd1", unet_spec.SD1, 16, False), ("sd1", unet_spec.SD1, 40, True)]
 TINY_RUNS = [("tiny", unet_spec.TINY, 2, False), ("tiny", unet_spec.TINY, 3, True)]
+# (part, config, chunk batch): the VAE runs ``decode_batch`` = 2 images per chunk (a sampling batch of 8 is four
+# chunks), and a batch of odd size ends with a chunk of 1
+VAE_RUNS = [("decoder", vae_mod.SD_VAE, 2), ("decoder", vae_mod.SD_VAE, 1),
+            ("encoder", vae_mod.SD_VAE, 2), ("encoder", vae_mod.SD_VAE, 1)]
+VAE_MICRO_RUNS = [("decoder", vae_mod.VAE_MICRO, 2), ("decoder", vae_mod.VAE_MICRO, 1),
+                  ("encoder", vae_mod.VAE_MICRO, 2), ("encoder", vae_mod.VAE_MICRO, 1)]
 
 PASS_THROUGH = ("gn_stats_shape", "groupnorm_workspace_floats")
 
@@ -41,15 +49,18 @@ class Tensor:
 
 
 class Call:
-    """one launch: ``args`` maps the op's parameter names to scalars, ``Tensor``s or None; ``batch`` is the U-Net batch of
-    the run, ``group_table`` the (w_off, b_off, y_off, n) entries of a dense_small_grouped launch"""
+    """one launch: ``args`` maps the op's parameter names to scalars, ``Tensor``s or None; ``batch`` is the number of
+    samples the launch covers (the U-Net batch, the VAE chunk, 1 inside the VAE attention's per-sample loop),
+    ``group_table`` the (w_off, b_off, y_off, n) entries of a dense_small_grouped launch, ``role`` what a VAE attention
+    GEMM computes ("vt": V^T = Wv^T g^T, "qk": Q K^T, "pv": P V), whose operands are not a weight and activations"""
 
-    def __init__(self, op, args, batch, group_table=None):
-        self.op, self.args, self.batch, self.group_table = op, args, batch, group_table
+    def __init__(self, op, args, batch, group_table=None, role=None):
+        self.op, self.args, self.batch, self.group_table, self.role = op, args, batch, group_table, role
 
     def key(self):
         items = tuple((k, v.key() if isinstance(v, Tensor) else v) for k, v in sorted(self.args.items()))
-        return (self.op, items, tuple(self.group_table) if self.group_table else None)
+        key = (self.op, items, tuple(self.group_table) if self.group_table else None)
+        return key + (self.role,) if self.role else key
 
     def tag(self):
         """a short readable name of the configuration (test ids)"""
@@ -61,13 +72,15 @@ class Call:
             flags = [f for f in ("bias", "rowvec", "residual", "out_f32", "out_bf16", "aux_bf16", "gn_stats")
                      if t(f) is not None]
             kind = f"conv{a.get('taps', 1)}s{a.get('stride', 1)}" if a.get("conv") else "lin"
+            kind = self.role or kind + ("-nolowpad" if a.get("no_low_pad") else "")
             return f"{kind}-M{rows}-N{a['n']}-K{k}" + ("-geglu" if a.get("geglu") else "") + "-" + "+".join(flags)
         if self.op == "attention_fwd":
             hd = a.get("head_dim", 64)
             return f"B{a['batch']}-H{a['heads']}-d{hd}-nq{a['nq']}-nk{a['nk']}" + ("-lse" if t("lse") else "")
         if self.op == "groupnorm_fwd":
             outs = "+".join(f for f in ("y_bf16", "y_f32", "raw_bf16", "stats0") if t(f) is not None)
-            return f"B{a['batch']}-hw{a['hw']}-c{a['c0']}+{a.get('c1', 0)}-silu{int(a.get('silu', True))}-{outs}"
+            eps = f"-eps{a['eps']:g}" if "eps" in a else ""
+            return f"B{a['batch']}-hw{a['hw']}-c{a['c0']}+{a.get('c1', 0)}-silu{int(a.get('silu', True))}{eps}-{outs}"
         if self.op == "layernorm_fwd":
             return f"m{a['m']}-c{a['c']}"
         first = next(v for v in a.values() if isinstance(v, Tensor))
@@ -86,6 +99,7 @@ class _Recorder:
         self.calls = []
         self.recording = False
         self.params = None
+        self.weights = None      # ids of a VAE's prepared GEMM weights: tells the attention's per-sample GEMMs apart
         self._tables = {}
 
     def dense_small_group_table(self, entries, device):
@@ -120,8 +134,23 @@ class _Recorder:
                     buf = bases.setdefault(id(base), len(bases))
                     off = v.storage_offset() - firsts.setdefault(buf, v.storage_offset())
                 out[k] = Tensor(tuple(v.shape), v.dtype, tuple(v.stride()), buf, off)
-            self.calls.append(Call(name, out, self.batch, table))
+            role, batch = self._vae_role(name, bound)
+            self.calls.append(Call(name, out, batch, table, role))
         return record
+
+    def _vae_role(self, name, bound):
+        """(role, samples covered): the VAE attention runs its score GEMMs and softmax once per sample, whatever the
+        chunk batch"""
+        if self.weights is None:
+            return None, self.batch
+        if name == "softmax_rows":
+            return None, 1
+        if name == "igemm":
+            if id(bound["a0"]) in self.weights:
+                return "vt", 1
+            if id(bound["wt"]) not in self.weights:
+                return ("qk" if bound.get("out_f32") is not None else "pv"), 1
+        return None, self.batch
 
 
 def _record_run(cfg, batch, taped):
@@ -151,15 +180,56 @@ def runs(which="full"):
     return {(name, b, taped): _record_run(cfg, b, taped) for name, cfg, b, taped in (RUNS if which == "full" else TINY_RUNS)}
 
 
+def _distinct(calls):
+    """[(signature key, Call, number of launches)] in first-launch order; launches that share a signature cover the same
+    number of samples"""
+    seen = {}
+    for c in calls:
+        k = c.key()
+        if k in seen:
+            assert seen[k][1].batch == c.batch, (c.test_id(), seen[k][1].batch, c.batch)
+            seen[k][2] += 1
+        else:
+            seen[k] = [k, c, 1]
+    return [tuple(v) for v in seen.values()]
+
+
 @functools.lru_cache(maxsize=None)
 def census(which="full"):
     """the distinct configurations, in first-launch order: [(signature key, Call, number of launches)]"""
-    seen = {}
-    for ctx_calls, fwd_calls in runs(which).values():
-        for c in ctx_calls + fwd_calls:
-            k = c.key()
-            if k in seen:
-                seen[k][2] += 1
-            else:
-                seen[k] = [k, c, 1]
-    return [tuple(v) for v in seen.values()]
+    return _distinct(c for ctx_calls, fwd_calls in runs(which).values() for c in ctx_calls + fwd_calls)
+
+
+def _record_vae_run(part, cfg, batch):
+    rec = _Recorder()
+    saved = vae_mod.ops
+    vae_mod.ops = rec
+    try:
+        cls = vae_mod.VAEDecoder if part == "decoder" else vae_mod.VAEEncoder
+        _, total = vae_mod.param_offsets(cfg, part=part)
+        net = cls(cfg, torch.empty(total, device="meta"), device="meta", decode_batch=batch)
+        rec.params = net.params if net.params._base is None else net.params._base
+        rec.weights = {id(t) for t in net.w.values()}
+        rec.batch, rec.recording = batch, True
+        s = cfg.sample_size
+        up = 2 ** (len(cfg.block_out_channels) - 1)
+        if part == "decoder":
+            net.decode(torch.empty(batch, cfg.latent_channels, s, s, device="meta"))
+        else:
+            net.encode(torch.empty(batch, s * up, s * up, cfg.out_channels, device="meta"))
+    finally:
+        vae_mod.ops = saved
+    return rec.calls
+
+
+@functools.lru_cache(maxsize=None)
+def vae_runs(which="full"):
+    """{(part, chunk batch): the launches of one chunk}"""
+    return {(part, b): _record_vae_run(part, cfg, b)
+            for part, cfg, b in (VAE_RUNS if which == "full" else VAE_MICRO_RUNS)}
+
+
+@functools.lru_cache(maxsize=None)
+def vae_census(which="full"):
+    """the VAE's distinct configurations (``census`` of the decoder and encoder runs)"""
+    return _distinct(c for calls in vae_runs(which).values() for c in calls)
