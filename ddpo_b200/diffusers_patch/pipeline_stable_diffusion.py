@@ -17,6 +17,7 @@ import numpy as np
 import torch
 
 from .. import ops
+from ..ops import graph_step   # host-side control: stays the real one where ``ops`` is swapped for an emulator
 from ..unet import UNet
 from .scheduling_ddim import DDIMScheduler
 
@@ -52,8 +53,7 @@ class StableDiffusionPipeline:
                 lat_in=torch.empty(2 * b, 4, h, w, device=dev), x_cur=torch.empty(b, n, device=dev),
                 x_next=torch.empty(b, n, device=dev), logp=torch.empty(b, device=dev),
                 eps=torch.empty(2 * b, 4, h, w, device=dev), t_dev=torch.zeros(1, dtype=torch.int32, device=dev),
-                key_dev=torch.zeros(2, dtype=torch.int32, device=dev), ws=ops.ddim_workspace(b, dev), graph=None,
-                sig=None)
+                key_dev=torch.zeros(2, dtype=torch.int32, device=dev), ws=ops.ddim_workspace(b, dev), graph=None)
         return self._graphs[key]
 
     def _one_step(self, S, b, state, ratio, guidance_scale, eta):
@@ -109,22 +109,15 @@ class StableDiffusionPipeline:
 
         S = self._step_buffers(b, h, w, dev)
         sig = (float(guidance_scale), float(eta), T, id(state.common.alphas_cumprod), self.scheduler.config.prediction_type)
+
+        def step():
+            self._one_step(S, b, state, ratio, float(guidance_scale), float(eta))
+
         S["x_cur"].copy_(traj[0])
         for s in range(T):
             S["t_dev"].copy_(ts_dev[s:s + 1])
             S["key_dev"].copy_(keys_dev[s])
-            if not self.use_cuda_graph:
-                self._one_step(S, b, state, ratio, float(guidance_scale), float(eta))
-            else:
-                if S["graph"] is None or S["sig"] != sig:
-                    # warm-up (fills the arena, sets kernel attributes), then capture
-                    self._one_step(S, b, state, ratio, float(guidance_scale), float(eta))
-                    torch.cuda.synchronize()
-                    g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g):
-                        self._one_step(S, b, state, ratio, float(guidance_scale), float(eta))
-                    S["graph"], S["sig"] = g, sig
-                S["graph"].replay()
+            S["graph"] = graph_step(S["graph"], sig, step, self.use_cuda_graph)
             traj[s + 1].copy_(S["x_next"])
             logps[s].copy_(S["logp"])
             S["x_cur"].copy_(S["x_next"])

@@ -8,37 +8,37 @@ import ctypes as C
 import numpy as np
 import torch
 
-from . import _lib
-from ._lib import AttentionArgs, DdimCommon, GroupNormArgs, IGemmArgs, check, lib
+from ._lib import AttentionArgs, AttentionBwdArgs, DdimCommon, GroupNormArgs, IGemmArgs, WgradArgs, check, lib
 
 DDIM_CHUNKS = 8
 
 # ---- instrumentation (bench.py): kernel-launch counter and optional CUDA-event profile ----
 LAUNCH_COUNT = 0           # kernels launched through this module since import
 PROFILE = None             # list of (name, work, event0, event1) while profiling, else None
-_KERNELS_PER_CALL = {"groupnorm_fwd": 2, "groupnorm_bwd": 3, "layernorm_bwd": 2}   # groupnorm_fwd: finalize + apply
-
-
 PROFILE_TAGS = []          # parallel to PROFILE: a shape tag per entry (bench.py --shapes)
+# kernels per call where it is not one; approximate (groupnorm_fwd launches one to three: statistics, finalize, apply)
+_KERNELS_PER_CALL = {"groupnorm_fwd": 2, "groupnorm_bwd": 3, "layernorm_bwd": 2, "attention_bwd": 3, "colsum_cast": 2,
+                     "conv_out_bwd": 3, "conv_in_wgrad": 2, "dense_small_bwd": 3, "grad_sumsq": 2, "wgrad": 2,
+                     "colsum_bf16": 2, "clip_adafactor": 5, "lora_grad": 2}
 
 
-def _run(name, status, work=0.0, ev=None, tag=""):
+def _launch(name, *args, work=0.0, tag="", symbol=None):
+    """``ddpo_<symbol or name>(*args, stream)`` on the current stream: counts its kernels and checks its status.  While
+    ``PROFILE`` is a list, CUDA events bracket the call, which is recorded as ``name`` with ``work`` and the shape tag
+    ``tag`` (callers build a tag only while profiling)."""
     global LAUNCH_COUNT
+    e0 = None
+    if PROFILE is not None:
+        e0 = torch.cuda.Event(enable_timing=True)
+        e0.record()
+    status = getattr(lib(), "ddpo_" + (symbol or name))(*args, _stream())
     LAUNCH_COUNT += _KERNELS_PER_CALL.get(name, 1)
-    if ev is not None:
+    if e0 is not None:
         e1 = torch.cuda.Event(enable_timing=True)
         e1.record()
-        PROFILE.append((name, work, ev, e1))
+        PROFILE.append((name, work, e0, e1))
         PROFILE_TAGS.append(tag)
     check(status, name)
-
-
-def _ev():
-    if PROFILE is None:
-        return None
-    e0 = torch.cuda.Event(enable_timing=True)
-    e0.record()
-    return e0
 
 
 def _stream():
@@ -54,6 +54,49 @@ def _p(t):
 
 def _chk(t, dtype, name):
     assert t.is_cuda and t.dtype == dtype and t.is_contiguous(), f"{name}: need contiguous CUDA {dtype}, got {t.dtype} {t.device}"
+
+
+# ---- scratch workspaces of the kernels that plan their own (wgrad, colsum, stems, LoRA), grown on demand ----
+# kind -> device -> fp32 tensor
+_WORKSPACES = {kind: {} for kind in ("wgrad", "colsum", "conv_out_bwd", "conv_in_wgrad", "lora_grad")}
+_WGRAD_WS = _WORKSPACES["wgrad"]   # the wgrad tests swap a workspace of their own in here
+
+
+def _workspace(kind, device, need, min_floats=1 << 20):
+    """The fp32 workspace of ``kind`` on ``device``: at least ``need`` floats.  One that is too small is replaced by
+    a new one of max(need, min_floats) floats; a CUDA graph captured with the old one keeps it (``graph_step``)."""
+    cache = _WORKSPACES[kind]
+    ws = cache.get(device)
+    if ws is None or ws.numel() < need:
+        ws = cache[device] = torch.empty(max(need, min_floats), dtype=torch.float32, device=device)
+    return ws
+
+
+def graph_step(captured, sig, body, enabled, protect=None):
+    """Run ``body()``, one step of kernels on fixed buffers, as the replay of a CUDA graph (eagerly when not
+    ``enabled``).  ``captured`` is what the previous call for these buffers returned, None at first.  Without a graph,
+    or with one captured at another ``sig``, the body first runs eagerly (the warm-up grows the arena and the
+    workspaces and sets kernel attributes; ``protect``, e.g. a gradient accumulator, gets its contents back after it)
+    and is then captured.
+
+    Returns what to pass next time: the signature, the graph and the workspaces it was captured with.  Holding those
+    keeps a workspace that ``_workspace`` has since replaced alive exactly as long as a graph that writes to it."""
+    if not enabled:
+        body()
+        return captured
+    if captured is None or captured[0] != sig:
+        saved = protect.clone() if protect is not None else None
+        body()
+        torch.cuda.synchronize()
+        if protect is not None:
+            protect.copy_(saved)
+        del saved   # a full gradient copy: freed before the capture allocates
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            body()
+        captured = (sig, graph, [ws for cache in _WORKSPACES.values() for ws in cache.values()])
+    captured[1].replay()
+    return captured
 
 
 # ------------------------------------------------------------------ PRNG --------
@@ -88,8 +131,7 @@ def key_tensor(keys, device):
 
 def threefry_normal(key_dev, out):
     _chk(out, torch.float32, "out")
-    _e = _ev()
-    _run("threefry_normal", lib().ddpo_threefry_normal(_p(key_dev), _p(out), out.numel(), _stream()), 0.0, _e)
+    _launch("threefry_normal", _p(key_dev), _p(out), out.numel())
     return out
 
 
@@ -126,28 +168,24 @@ def _ddim_common(eps_u, eps_c, sample, alphas_cumprod, timesteps, final_alpha, s
 def ddim_step_sample(eps_u, eps_c, sample, alphas_cumprod, timesteps, final_alpha, step_ratio, guidance, eta,
                      key_dev, prev_out, logp_out, ws, pred="epsilon"):
     c = _ddim_common(eps_u, eps_c, sample, alphas_cumprod, timesteps, final_alpha, step_ratio, guidance, eta, ws, pred)
-    _e = _ev()
-    _run("ddim_step_sample", lib().ddpo_ddim_step_sample(C.byref(c), _p(key_dev), _p(prev_out), _p(logp_out), _stream()), 0.0, _e)
+    _launch("ddim_step_sample", C.byref(c), _p(key_dev), _p(prev_out), _p(logp_out))
 
 
 def ddim_logprob_fwd(eps_u, eps_c, sample, prev, alphas_cumprod, timesteps, final_alpha, step_ratio, guidance, eta,
                      logp_out, ws, pred="epsilon"):
     c = _ddim_common(eps_u, eps_c, sample, alphas_cumprod, timesteps, final_alpha, step_ratio, guidance, eta, ws, pred)
-    _e = _ev()
-    _run("ddim_logprob_fwd", lib().ddpo_ddim_logprob_fwd(C.byref(c), _p(prev), _p(logp_out), _stream()), 0.0, _e)
+    _launch("ddim_logprob_fwd", C.byref(c), _p(prev), _p(logp_out))
 
 
 def ddim_logprob_bwd(eps_u, eps_c, sample, prev, alphas_cumprod, timesteps, final_alpha, step_ratio, guidance, eta,
                      dlogp, d_eps_u, d_eps_c, ws, pred="epsilon"):
     c = _ddim_common(eps_u, eps_c, sample, alphas_cumprod, timesteps, final_alpha, step_ratio, guidance, eta, ws, pred)
-    _e = _ev()
-    _run("ddim_logprob_bwd", lib().ddpo_ddim_logprob_bwd(C.byref(c), _p(prev), _p(dlogp), _p(d_eps_u), _p(d_eps_c), _stream()), 0.0, _e)
+    _launch("ddim_logprob_bwd", C.byref(c), _p(prev), _p(dlogp), _p(d_eps_u), _p(d_eps_c))
 
 
 def ppo_loss(logp, old_logp, adv, clip_range, info_out, dlogp_out, micro_batch=None):
-    _e = _ev()
-    _run("ppo_loss", lib().ddpo_ppo_loss(_p(logp), _p(old_logp), _p(adv), logp.numel(), int(micro_batch or logp.numel()),
-                                         float(clip_range), _p(info_out), _p(dlogp_out), _stream()), 0.0, _e)
+    _launch("ppo_loss", _p(logp), _p(old_logp), _p(adv), logp.numel(), int(micro_batch or logp.numel()), float(clip_range),
+            _p(info_out), _p(dlogp_out))
 
 
 # ------------------------------------------------------------------ GEMM --------
@@ -178,11 +216,11 @@ def igemm(*, a0, wt, n, a1=None, c0=None, c1=0, lda0=None, lda1=None, conv=None,
     a.gn_stats = _p(gn_stats)
     a.conv_pad = int(no_low_pad)
     rows = a.batch * a.h * a.w if a.is_conv else a.m
-    _e = _ev()
-    _run("igemm", lib().ddpo_igemm(C.byref(a), _stream()), 2.0 * rows * a.n * a.taps * (a.c0 + a.c1), _e,
-         f"M{rows} N{a.n} K{a.taps * (a.c0 + a.c1)} taps{a.taps} s{a.conv_stride}"
-         f"{' geglu' if geglu else ''}{' res' if residual is not None else ''}{' f32' if out_f32 is not None else ''}"
-         f"{' bf16' if out_bf16 is not None else ''}{' acc' if accumulate else ''}" if _e is not None else "")
+    _launch("igemm", C.byref(a), work=2.0 * rows * a.n * a.taps * (a.c0 + a.c1),
+            tag=f"M{rows} N{a.n} K{a.taps * (a.c0 + a.c1)} taps{a.taps} s{a.conv_stride}"
+                f"{' geglu' if geglu else ''}{' res' if residual is not None else ''}"
+                f"{' f32' if out_f32 is not None else ''}{' bf16' if out_bf16 is not None else ''}"
+                f"{' acc' if accumulate else ''}" if PROFILE is not None else "")
 
 
 # ------------------------------------------------------------------ norms -------
@@ -208,9 +246,8 @@ def groupnorm_fwd(x0, scale, bias, ws, batch, hw, c0, x1=None, c1=0, silu=True, 
     (or ``stats0`` alone for one source) and hw % 32 == 0 the statistics pass over x is skipped."""
     a = _gn_args(x0, x1, c0, c1, batch, hw, scale, bias, silu, y_bf16, y_f32, raw_bf16, ws, skip_stats=skip_stats,
                  eps=eps, stats0=stats0, stats1=stats1)
-    _e = _ev()
     per = 4 + (2 if y_bf16 is not None else 0) + (4 if y_f32 is not None else 0) + (2 if raw_bf16 is not None else 0)
-    _run("groupnorm_fwd", lib().ddpo_groupnorm_fwd(C.byref(a), _stream()), float(batch) * hw * (c0 + c1) * per, _e)
+    _launch("groupnorm_fwd", C.byref(a), work=float(batch) * hw * (c0 + c1) * per)
 
 
 def groupnorm_bwd(x0, scale, bias, ws, batch, hw, c0, dy, dx0, dscale, dbias, x1=None, c1=0, dx1=None, silu=True,
@@ -218,14 +255,12 @@ def groupnorm_bwd(x0, scale, bias, ws, batch, hw, c0, dy, dx0, dscale, dbias, x1
     """``dy`` fp32 or bf16 (the dtype selects the kernel's load path): the dgrad GEMM in front of a GroupNorm writes bf16."""
     assert dy.dtype in (torch.float32, torch.bfloat16)
     a = _gn_args(x0, x1, c0, c1, batch, hw, scale, bias, silu, None, None, None, ws, dy_bf16=dy.dtype == torch.bfloat16)
-    _e = _ev()
-    _run("groupnorm_bwd", lib().ddpo_groupnorm_bwd(C.byref(a), _p(dy), _p(dx0), _p(dx1), int(ldd0), int(ldd1), int(accumulate),
-                                   _p(dscale), _p(dbias), _stream()), 0.0, _e)
+    _launch("groupnorm_bwd", C.byref(a), _p(dy), _p(dx0), _p(dx1), int(ldd0), int(ldd1), int(accumulate), _p(dscale),
+            _p(dbias))
 
 
 def layernorm_fwd(x, scale, bias, y_bf16, m, c, stats=None):
-    _e = _ev()
-    _run("layernorm_fwd", lib().ddpo_layernorm_fwd(_p(x), _p(scale), _p(bias), _p(y_bf16), _p(stats), int(m), int(c), 1e-5, _stream()), 0.0, _e)
+    _launch("layernorm_fwd", _p(x), _p(scale), _p(bias), _p(y_bf16), _p(stats), int(m), int(c), 1e-5)
 
 
 def layernorm_bwd_workspace_floats(m, c):
@@ -234,68 +269,54 @@ def layernorm_bwd_workspace_floats(m, c):
 
 def layernorm_bwd(x, scale, stats, dy, dx, dscale, dbias, ws, m, c, accumulate=False):
     assert dy.dtype in (torch.float32, torch.bfloat16)
-    _e = _ev()
-    _run("layernorm_bwd", lib().ddpo_layernorm_bwd(_p(x), _p(scale), _p(stats), _p(dy), _p(dx), int(accumulate), _p(dscale),
-                                   _p(dbias), _p(ws), int(m), int(c), int(dy.dtype == torch.bfloat16), _stream()), 0.0, _e)
+    _launch("layernorm_bwd", _p(x), _p(scale), _p(stats), _p(dy), _p(dx), int(accumulate), _p(dscale), _p(dbias), _p(ws),
+            int(m), int(c), int(dy.dtype == torch.bfloat16))
 
 
 # ------------------------------------------------------------ small layers -------
 def prep_weight(src, dst, k, n, ldk=None, row_offset=0, col_offset=0, geglu_bn=0):
-    _e = _ev()
-    _run("prep_weight", lib().ddpo_prep_weight(_p(src), _p(dst), int(k), int(n), int(ldk or k), int(row_offset), int(col_offset),
-                                 int(geglu_bn), _stream()), 0.0, _e)
+    _launch("prep_weight", _p(src), _p(dst), int(k), int(n), int(ldk or k), int(row_offset), int(col_offset),
+            int(geglu_bn))
 
 
 def prep_weight_dgrad(src, dst, taps, k, n, ld_dst=0, col_offset=0):
-    _e = _ev()
-    _run("prep_weight_dgrad", lib().ddpo_prep_weight_dgrad(_p(src), _p(dst), int(taps), int(k), int(n), int(ld_dst),
-                                                           int(col_offset), _stream()), 0.0, _e)
+    _launch("prep_weight_dgrad", _p(src), _p(dst), int(taps), int(k), int(n), int(ld_dst), int(col_offset))
 
 
 def permute_geglu_bias(src, dst, n, bn):
-    _e = _ev()
-    _run("permute_geglu_bias", lib().ddpo_permute_geglu_bias(_p(src), _p(dst), int(n), int(bn), _stream()), 0.0, _e)
+    _launch("permute_geglu_bias", _p(src), _p(dst), int(n), int(bn))
 
 
 def cast_bf16(x, y):
-    _e = _ev()
-    _run("cast_bf16", lib().ddpo_cast_bf16(_p(x), _p(y), x.numel(), _stream()), 0.0, _e)
+    _launch("cast_bf16", _p(x), _p(y), x.numel())
 
 
 def upsample2x_bf16(x, y, batch, h, w, c):
-    _e = _ev()
-    _run("upsample2x_bf16", lib().ddpo_upsample2x_bf16(_p(x), _p(y), batch, h, w, c, _stream()), 0.0, _e)
+    _launch("upsample2x_bf16", _p(x), _p(y), batch, h, w, c)
 
 
 def upsample2x_bwd(dy, dx, batch, h, w, c, accumulate=False):
-    _e = _ev()
-    _run("upsample2x_bwd", lib().ddpo_upsample2x_bwd(_p(dy), _p(dx), batch, h, w, c, int(accumulate), _stream()), 0.0, _e)
+    _launch("upsample2x_bwd", _p(dy), _p(dx), batch, h, w, c, int(accumulate))
 
 
 def conv_in(x_nchw, w, bias, y_nhwc, batch, cin, h, wd, cout, gn_stats=None):
-    _e = _ev()
-    _run("conv_in", lib().ddpo_conv_in(_p(x_nchw), _p(w), _p(bias), _p(y_nhwc), batch, cin, h, wd, cout, _p(gn_stats),
-                                       _stream()), 0.0, _e)
+    _launch("conv_in", _p(x_nchw), _p(w), _p(bias), _p(y_nhwc), batch, cin, h, wd, cout, _p(gn_stats))
 
 
 def conv_out(x_nhwc, w, bias, y_nchw, batch, h, wd, cin, cout):
-    _e = _ev()
-    _run("conv_out", lib().ddpo_conv_out(_p(x_nhwc), _p(w), _p(bias), _p(y_nchw), batch, h, wd, cin, cout, _stream()), 0.0, _e)
+    _launch("conv_out", _p(x_nhwc), _p(w), _p(bias), _p(y_nchw), batch, h, wd, cin, cout)
 
 
 def timestep_sincos(t, out, batch, dim):
-    _e = _ev()
-    _run("timestep_sincos", lib().ddpo_timestep_sincos(_p(t), 1 if t.numel() > 1 else 0, _p(out), batch, dim, _stream()), 0.0, _e)
+    _launch("timestep_sincos", _p(t), 1 if t.numel() > 1 else 0, _p(out), batch, dim)
 
 
 def dense_small(x, w, bias, y, batch, k, n, silu_in=False, silu_out=False):
-    _e = _ev()
-    _run("dense_small", lib().ddpo_dense_small(_p(x), _p(w), _p(bias), _p(y), batch, k, n, int(silu_in), int(silu_out), _stream()), 0.0, _e)
+    _launch("dense_small", _p(x), _p(w), _p(bias), _p(y), batch, k, n, int(silu_in), int(silu_out))
 
 
 def dense_small_group_table(entries, device):
     """entries: [(w_off, bias_off, y_off, n)] in floats -> (device uint8 table, total CTAs) for dense_small_grouped."""
-    import numpy as np
     rec = np.zeros(len(entries), dtype=[("w", "<i8"), ("b", "<i8"), ("y", "<i8"), ("n", "<i4"), ("cta0", "<i4")])
     cta = 0
     for i, (w_off, b_off, y_off, n) in enumerate(entries):
@@ -305,9 +326,8 @@ def dense_small_group_table(entries, device):
 
 
 def dense_small_grouped(x, params_base, y_base, table, n_groups, total_ctas, batch, k):
-    _e = _ev()
-    _run("dense_small", lib().ddpo_dense_small_grouped(_p(x), _p(params_base), _p(y_base), _p(table), int(n_groups),
-                                                       int(total_ctas), int(batch), int(k), _stream()), 0.0, _e)
+    _launch("dense_small", _p(x), _p(params_base), _p(y_base), _p(table), int(n_groups), int(total_ctas), int(batch),
+            int(k), symbol="dense_small_grouped")
 
 
 # --------------------------------------------------------------- attention -------
@@ -318,18 +338,13 @@ def attention_fwd(q, k, v, out, batch, heads, nq, nk, ldq, ldk, ldv, ldo, lse=No
     """head h of q/k/v/out at columns [h * head_dim, (h + 1) * head_dim); head_dim is 40, 64, 80 or 160"""
     a = AttentionArgs(_p(q), _p(k), _p(v), _p(out), _p(lse), batch, heads, nq, nk, head_dim, ldq, ldk, ldv, ldo,
                       int(causal))
-    _e = _ev()
-    _run("attention_fwd", lib().ddpo_attention_fwd(C.byref(a), _stream()), 4.0 * batch * heads * nq * nk * head_dim, _e,
-         f"B{batch} H{heads} nq{nq} nk{nk}")
+    _launch("attention_fwd", C.byref(a), work=4.0 * batch * heads * nq * nk * head_dim,
+            tag=f"B{batch} H{heads} nq{nq} nk{nk}" if PROFILE is not None else "")
 
 
 # ------------------------------------------------------------------ wgrad -------
-_WGRAD_WS = {}
-
-
 def wgrad(*, dy, n, x0, dw, x1=None, c0=None, c1=0, ldy=0, ldx0=0, ldx1=0, conv=None, m=None, taps=1, stride=1):
     """dw[(tap, cin), n] += X^T dY (fp32, Flax layout).  conv=(batch, h_out, w_out) or linear with m rows."""
-    from ._lib import WgradArgs
     a = WgradArgs()
     a.dy, a.ldy, a.n = _p(dy), int(ldy), int(n)
     a.x0, a.x1 = _p(x0), _p(x1)
@@ -342,35 +357,21 @@ def wgrad(*, dy, n, x0, dw, x1=None, c0=None, c1=0, ldy=0, ldx0=0, ldx1=0, conv=
     a.conv_stride, a.taps = int(stride), int(taps)
     a.dw = _p(dw)
     need = int(lib().ddpo_wgrad_workspace_floats(C.byref(a)))
-    dev = dw.device
-    ws = _WGRAD_WS.get(dev)
-    if need > 0 and (ws is None or ws.numel() < need):
-        ws = torch.empty(max(need, 1 << 20), dtype=torch.float32, device=dev)
-        _WGRAD_WS[dev] = ws
-    a.workspace = _p(ws) if need > 0 else None
-    a.workspace_floats = ws.numel() if (need > 0) else 0
+    ws = _workspace("wgrad", dw.device, need) if need > 0 else None
+    a.workspace = _p(ws)
+    a.workspace_floats = ws.numel() if ws is not None else 0
     rows = a.batch * a.h * a.w if a.is_conv else a.m
-    _e = _ev()
-    _run("wgrad", lib().ddpo_wgrad(C.byref(a), _stream()), 2.0 * rows * a.n * a.taps * (a.c0 + a.c1), _e,
-         f"M{rows} N{a.n} K{a.taps * (a.c0 + a.c1)} taps{a.taps} s{a.conv_stride}")
+    _launch("wgrad", C.byref(a), work=2.0 * rows * a.n * a.taps * (a.c0 + a.c1),
+            tag=f"M{rows} N{a.n} K{a.taps * (a.c0 + a.c1)} taps{a.taps} s{a.conv_stride}" if PROFILE is not None else "")
 
 
 # ------------------------------------------------------- backward wrappers -------
 def attention_bwd(q, k, v, out, dout, lse, delta, dq, dk, dv, batch, heads, nq, nk, ldq, ldk, ldv, ldo, lddo, lddq,
                   lddk, lddv, head_dim=64):
-    from ._lib import AttentionBwdArgs
     a = AttentionBwdArgs(_p(q), _p(k), _p(v), _p(out), _p(dout), _p(lse), _p(delta), _p(dq), _p(dk), _p(dv), batch,
                          heads, nq, nk, head_dim, ldq, ldk, ldv, ldo, lddo, lddq, lddk, lddv)
-    _e = _ev()
-    _run("attention_bwd", lib().ddpo_attention_bwd(C.byref(a), _stream()), 14.0 * batch * heads * nq * nk * head_dim, _e,
-         f"B{batch} H{heads} nq{nq} nk{nk}")
-
-
-_CIW_WS = {}
-_KERNELS_PER_CALL.update({"attention_bwd": 3, "colsum_cast": 2, "conv_out_bwd": 3, "conv_in_wgrad": 2,
-                          "dense_small_bwd": 3, "grad_sumsq": 2, "wgrad": 2, "colsum_bf16": 2,
-                          "clip_adafactor": 5})
-_COLSUM_WS = {}
+    _launch("attention_bwd", C.byref(a), work=14.0 * batch * heads * nq * nk * head_dim,
+            tag=f"B{batch} H{heads} nq{nq} nk{nk}" if PROFILE is not None else "")
 
 
 def colsum_cast(dy, m, n, y_bf16=None, out=None, rows_per_group=None, accumulate=True, ld=0):
@@ -378,72 +379,42 @@ def colsum_cast(dy, m, n, y_bf16=None, out=None, rows_per_group=None, accumulate
     rpg = int(rows_per_group or m)
     ws = None
     if out is not None:
-        need = int(lib().ddpo_colsum_workspace_floats(m, n, rpg))
-        ws = _COLSUM_WS.get(dy.device)
-        if ws is None or ws.numel() < need:
-            ws = torch.empty(max(need, 1 << 20), dtype=torch.float32, device=dy.device)
-            _COLSUM_WS[dy.device] = ws
-    _e = _ev()
-    _run("colsum_cast", lib().ddpo_colsum_cast(_p(dy), int(ld), _p(y_bf16), _p(out), rpg, int(accumulate), _p(ws), int(m),
-                                               int(n), _stream()), float(m) * n * 6, _e)
+        ws = _workspace("colsum", dy.device, int(lib().ddpo_colsum_workspace_floats(m, n, rpg)))
+    _launch("colsum_cast", _p(dy), int(ld), _p(y_bf16), _p(out), rpg, int(accumulate), _p(ws), int(m), int(n),
+            work=float(m) * n * 6)
 
 
 def colsum_bf16(x, m, n, out, accumulate=True, ld=0):
-    need = int(lib().ddpo_colsum_workspace_floats(m, n, m))
-    ws = _COLSUM_WS.get(x.device)
-    if ws is None or ws.numel() < need:
-        ws = torch.empty(max(need, 1 << 20), dtype=torch.float32, device=x.device)
-        _COLSUM_WS[x.device] = ws
-    _e = _ev()
-    _run("colsum_bf16", lib().ddpo_colsum_bf16(_p(x), int(ld), _p(out), int(accumulate), _p(ws), int(m), int(n), _stream()),
-         float(m) * n * 2, _e)
+    ws = _workspace("colsum", x.device, int(lib().ddpo_colsum_workspace_floats(m, n, m)))
+    _launch("colsum_bf16", _p(x), int(ld), _p(out), int(accumulate), _p(ws), int(m), int(n), work=float(m) * n * 2)
 
 
 def geglu_bwd(pre, dff, dpre, m, n, bn=256):
     assert dff.dtype in (torch.float32, torch.bfloat16)
-    _e = _ev()
-    _run("geglu_bwd", lib().ddpo_geglu_bwd(_p(pre), _p(dff), _p(dpre), int(m), int(n), int(bn),
-                                           int(dff.dtype == torch.bfloat16), _stream()), 0.0, _e)
+    _launch("geglu_bwd", _p(pre), _p(dff), _p(dpre), int(m), int(n), int(bn), int(dff.dtype == torch.bfloat16))
 
 
 def conv_out_bwd(x_nhwc, w, dy_nchw, dx_nhwc, dw, dbias, batch, h, wd, cin):
-    need = int(lib().ddpo_conv_out_bwd_workspace_floats(cin))
-    ws = _CIW_WS.get(("cow", dw.device))
-    if ws is None or ws.numel() < need:
-        ws = torch.empty(need, dtype=torch.float32, device=dw.device)
-        _CIW_WS[("cow", dw.device)] = ws
-    _e = _ev()
-    _run("conv_out_bwd", lib().ddpo_conv_out_bwd(_p(x_nhwc), _p(w), _p(dy_nchw), _p(dx_nhwc), _p(dw), _p(dbias), _p(ws),
-                                                 batch, h, wd, cin, _stream()), 0.0, _e)
+    ws = _workspace("conv_out_bwd", dw.device, int(lib().ddpo_conv_out_bwd_workspace_floats(cin)), min_floats=0)
+    _launch("conv_out_bwd", _p(x_nhwc), _p(w), _p(dy_nchw), _p(dx_nhwc), _p(dw), _p(dbias), _p(ws), batch, h, wd, cin)
 
 
 def conv_in_wgrad(lat, dx_nhwc, dw, batch, cin, h, wd, cout):
-    need = int(lib().ddpo_conv_in_wgrad_workspace_floats(cin, cout))
-    ws = _CIW_WS.get(dw.device)
-    if ws is None or ws.numel() < need:
-        ws = torch.empty(need, dtype=torch.float32, device=dw.device)
-        _CIW_WS[dw.device] = ws
-    _e = _ev()
-    _run("conv_in_wgrad", lib().ddpo_conv_in_wgrad(_p(lat), _p(dx_nhwc), _p(dw), _p(ws), batch, cin, h, wd, cout,
-                                                   _stream()), 0.0, _e)
+    ws = _workspace("conv_in_wgrad", dw.device, int(lib().ddpo_conv_in_wgrad_workspace_floats(cin, cout)), min_floats=0)
+    _launch("conv_in_wgrad", _p(lat), _p(dx_nhwc), _p(dw), _p(ws), batch, cin, h, wd, cout)
 
 
 def dense_small_bwd(x, w, bias, dy, dpre_ws, dw, db, dx, batch, k, n, silu_in=False, silu_out=False, dx_accumulate=False):
-    _e = _ev()
-    _run("dense_small_bwd", lib().ddpo_dense_small_bwd(_p(x), _p(w), _p(bias), _p(dy), _p(dpre_ws), _p(dw), _p(db), _p(dx),
-                                                       int(dx_accumulate), batch, k, n, int(silu_in), int(silu_out),
-                                                       _stream()), 0.0, _e)
+    _launch("dense_small_bwd", _p(x), _p(w), _p(bias), _p(dy), _p(dpre_ws), _p(dw), _p(db), _p(dx), int(dx_accumulate),
+            batch, k, n, int(silu_in), int(silu_out))
 
 
 def dilate2x_bf16(x, y, batch, h, w, c):
-    _e = _ev()
-    _run("dilate2x_bf16", lib().ddpo_dilate2x_bf16(_p(x), _p(y), batch, h, w, c, _stream()), 0.0, _e)
+    _launch("dilate2x_bf16", _p(x), _p(y), batch, h, w, c)
 
 
 def copy2d(src, lds, dst, ldd, rows, cols, accumulate=False):
-    _e = _ev()
-    _run("copy2d", lib().ddpo_copy2d(_p(src), int(lds), _p(dst), int(ldd), int(rows), int(cols), int(accumulate),
-                                     _stream()), 0.0, _e)
+    _launch("copy2d", _p(src), int(lds), _p(dst), int(ldd), int(rows), int(cols), int(accumulate))
 
 
 def gather_rows(src, index, dst):
@@ -454,9 +425,7 @@ def gather_rows(src, index, dst):
     rows = index.numel()
     row_floats = dst.numel() // rows
     assert src.numel() % row_floats == 0 and dst.numel() == rows * row_floats
-    _e = _ev()
-    _run("gather_rows", lib().ddpo_gather_rows(_p(src), _p(index), _p(dst), rows, row_floats, _stream()),
-         float(rows) * row_floats * 8, _e)
+    _launch("gather_rows", _p(src), _p(index), _p(dst), rows, row_floats, work=float(rows) * row_floats * 8)
 
 
 def optim_workspace(device):
@@ -464,16 +433,13 @@ def optim_workspace(device):
 
 
 def grad_sumsq(g, ws, out):
-    _e = _ev()
-    _run("grad_sumsq", lib().ddpo_grad_sumsq(_p(g), g.numel(), _p(ws), _p(out), _stream()), float(g.numel()) * 4, _e)
+    _launch("grad_sumsq", _p(g), g.numel(), _p(ws), _p(out), work=float(g.numel()) * 4)
 
 
 def clip_adamw(params, grad_acc, mu, nu, sumsq, grad_scale, max_norm, lr, b1, b2, eps, wd, step, norm_out=None):
-    _e = _ev()
-    _run("clip_adamw", lib().ddpo_clip_adamw(_p(params), _p(grad_acc), _p(mu), _p(nu), params.numel(), _p(sumsq),
-                                             float(grad_scale), float(max_norm), float(lr), float(b1), float(b2),
-                                             float(eps), float(wd), int(step), _p(norm_out), _stream()),
-         float(params.numel()) * 24, _e)
+    _launch("clip_adamw", _p(params), _p(grad_acc), _p(mu), _p(nu), params.numel(), _p(sumsq), float(grad_scale),
+            float(max_norm), float(lr), float(b1), float(b2), float(eps), float(wd), int(step), _p(norm_out),
+            work=float(params.numel()) * 24)
 
 
 class AdafactorPlan:
@@ -537,11 +503,9 @@ def clip_adafactor(params, grad_acc, state, plan, workspace, sumsq, grad_scale, 
     for t, nm in ((params, "params"), (grad_acc, "grad_acc"), (state, "state"), (workspace, "workspace")):
         _chk(t, torch.float32, nm)
     assert grad_acc.numel() == params.numel()
-    _e = _ev()
-    _run("clip_adafactor", lib().ddpo_clip_adafactor(
-        _p(params), _p(grad_acc), _p(state), state.numel(), params.numel(), plan.host.ctypes.data,
-        _p(plan.device_copy(params.device)), _p(workspace), workspace.numel(), _p(sumsq), float(grad_scale),
-        float(max_norm), float(lr), float(wd), int(step), _p(norm_out), _stream()), float(params.numel()) * 28, _e)
+    _launch("clip_adafactor", _p(params), _p(grad_acc), _p(state), state.numel(), params.numel(), plan.host.ctypes.data,
+            _p(plan.device_copy(params.device)), _p(workspace), workspace.numel(), _p(sumsq), float(grad_scale),
+            float(max_norm), float(lr), float(wd), int(step), _p(norm_out), work=float(params.numel()) * 28)
 
 
 # --------------------------------------------------------------------- RWR -------
@@ -558,11 +522,8 @@ def rwr_noisy_latents(moments_nhwc, key_sample_dev, key_noise_dev, timesteps, al
     _chk(noisy_out, torch.float32, "noisy_out")
     b, h, w, c2 = moments_nhwc.shape
     assert timesteps.numel() == b and noise_out.numel() == b * (c2 // 2) * h * w == noisy_out.numel()
-    _e = _ev()
-    _run("rwr_noisy_latents", lib().ddpo_rwr_noisy_latents(_p(moments_nhwc), _p(key_sample_dev), _p(key_noise_dev),
-                                                           _p(timesteps), _p(alphas_cumprod), float(scaling), b, c2 // 2,
-                                                           h, w, _p(noise_out), _p(noisy_out), _p(latents_out),
-                                                           _stream()), 0.0, _e)
+    _launch("rwr_noisy_latents", _p(moments_nhwc), _p(key_sample_dev), _p(key_noise_dev), _p(timesteps),
+            _p(alphas_cumprod), float(scaling), b, c2 // 2, h, w, _p(noise_out), _p(noisy_out), _p(latents_out))
 
 
 def rwr_mse_loss(eps_u, eps_c, noise, guidance, loss_out, ws, weights=None, per_sample=None, d_eps_u=None, d_eps_c=None):
@@ -574,10 +535,8 @@ def rwr_mse_loss(eps_u, eps_c, noise, guidance, loss_out, ws, weights=None, per_
     if weights is not None:
         _chk(weights, torch.float32, "weights")
         assert weights.numel() == b
-    _e = _ev()
-    _run("rwr_mse_loss", lib().ddpo_rwr_mse_loss(_p(eps_u), _p(eps_c), _p(noise), _p(weights), float(guidance), b, n,
-                                                 _p(loss_out), _p(per_sample), _p(d_eps_u), _p(d_eps_c), _p(ws),
-                                                 _stream()), 0.0, _e)
+    _launch("rwr_mse_loss", _p(eps_u), _p(eps_c), _p(noise), _p(weights), float(guidance), b, n, _p(loss_out),
+            _p(per_sample), _p(d_eps_u), _p(d_eps_c), _p(ws))
 
 
 # --------------------------------------------------------------------- VAE -------
@@ -585,9 +544,7 @@ def vae_post_quant(latents, w, bias, out, scaling=0.18215):
     _chk(latents, torch.float32, "latents")
     _chk(out, torch.float32, "out")
     b, c, h, wd = latents.shape
-    _e = _ev()
-    _run("vae_post_quant", lib().ddpo_vae_post_quant(_p(latents), _p(w), _p(bias), float(scaling), b, c, h, wd, _p(out),
-                                                     _stream()), 0.0, _e)
+    _launch("vae_post_quant", _p(latents), _p(w), _p(bias), float(scaling), b, c, h, wd, _p(out))
 
 
 def softmax_rows(scores, probs_bf16, scale):
@@ -595,9 +552,7 @@ def softmax_rows(scores, probs_bf16, scale):
     _chk(scores, torch.float32, "scores")
     _chk(probs_bf16, torch.bfloat16, "probs")
     rows, n = scores.shape
-    _e = _ev()
-    _run("softmax_rows", lib().ddpo_softmax_rows(_p(scores), n, float(scale), _p(probs_bf16), n, rows, n, _stream()),
-         float(rows) * n * 6, _e)
+    _launch("softmax_rows", _p(scores), n, float(scale), _p(probs_bf16), n, rows, n, work=float(rows) * n * 6)
 
 
 def image_to_uint8(img, out_u8):
@@ -605,8 +560,7 @@ def image_to_uint8(img, out_u8):
     _chk(img, torch.float32, "images")
     _chk(out_u8, torch.uint8, "out")
     assert img.numel() == out_u8.numel() and img.numel() % 4 == 0
-    _e = _ev()
-    _run("image_to_uint8", lib().ddpo_image_to_uint8(_p(img), _p(out_u8), img.numel(), _stream()), 0.0, _e)
+    _launch("image_to_uint8", _p(img), _p(out_u8), img.numel())
 
 
 # ------------------------------------------------- image-symmetry / consistency rewards -------
@@ -621,10 +575,8 @@ def resample_u8(src, transform, axis, table_host, table_dev, dst):
     n_out = table_host.shape[0]
     th, tw = (w, h) if transform in (2, 4) else (h, w)
     assert c == 3 and tuple(dst.shape) == ((b, th, n_out, 3) if axis == 0 else (b, n_out, tw, 3)), (src.shape, dst.shape)
-    _e = _ev()
-    _run("resample_u8", lib().ddpo_resample_u8(_p(src), b, h, w, int(transform), int(axis), n_out,
-                                               table_host.ctypes.data, _p(table_dev), table_host.shape[1] - 2, _p(dst),
-                                               _stream()), float(dst.numel() + src.numel()), _e)
+    _launch("resample_u8", _p(src), b, h, w, int(transform), int(axis), n_out, table_host.ctypes.data, _p(table_dev),
+            table_host.shape[1] - 2, _p(dst), work=float(dst.numel() + src.numel()))
 
 
 def clip_normalize_u8(src, top, left, out):
@@ -634,9 +586,7 @@ def clip_normalize_u8(src, top, left, out):
     b, h, w, _ = src.shape
     size = out.shape[1]
     assert tuple(out.shape) == (b, size, size, 3)
-    _e = _ev()
-    _run("clip_normalize_u8", lib().ddpo_clip_normalize_u8(_p(src), b, h, w, int(top), int(left), size, _p(out),
-                                                           _stream()), float(out.numel()) * 5, _e)
+    _launch("clip_normalize_u8", _p(src), b, h, w, int(top), int(left), size, _p(out), work=float(out.numel()) * 5)
 
 
 def pair_stats_u8(src, transform, out):
@@ -646,9 +596,7 @@ def pair_stats_u8(src, transform, out):
     _chk(out, torch.int64, "out")
     b, h, w, _ = src.shape
     assert tuple(out.shape) == (b, 4)
-    _e = _ev()
-    _run("pair_stats_u8", lib().ddpo_pair_stats_u8(_p(src), b, h, w, int(transform), _p(out), _stream()),
-         float(src.numel()) * 2, _e)
+    _launch("pair_stats_u8", _p(src), b, h, w, int(transform), _p(out), work=float(src.numel()) * 2)
 
 
 def feature_angles(feats, variants, out):
@@ -657,9 +605,7 @@ def feature_angles(feats, variants, out):
     _chk(out, torch.float32, "out")
     n = out.numel()
     assert feats.dim() == 2 and feats.shape[0] == variants * n
-    _e = _ev()
-    _run("feature_angles", lib().ddpo_feature_angles(_p(feats), int(variants), n, feats.shape[1], _p(out), _stream()),
-         float(feats.numel()) * 4, _e)
+    _launch("feature_angles", _p(feats), int(variants), n, feats.shape[1], _p(out), work=float(feats.numel()) * 4)
 
 
 def scaled_cosine(img, txt, logit_scale, out):
@@ -668,9 +614,8 @@ def scaled_cosine(img, txt, logit_scale, out):
     _chk(txt, torch.float32, "txt")
     _chk(out, torch.float32, "out")
     assert img.shape == txt.shape and img.dim() == 2 and out.numel() == img.shape[0]
-    _e = _ev()
-    _run("scaled_cosine", lib().ddpo_scaled_cosine(_p(img), _p(txt), img.shape[0], img.shape[1], float(logit_scale),
-                                                   _p(out), _stream()), float(img.numel()) * 8, _e)
+    _launch("scaled_cosine", _p(img), _p(txt), img.shape[0], img.shape[1], float(logit_scale), _p(out),
+            work=float(img.numel()) * 8)
 
 
 def vae_image_to_nchw(img_nhwc, out_nchw):
@@ -678,21 +623,16 @@ def vae_image_to_nchw(img_nhwc, out_nchw):
     _chk(out_nchw, torch.float32, "out")
     b, h, w, c = img_nhwc.shape
     assert c == 3 and tuple(out_nchw.shape) == (b, 3, h, w)
-    _e = _ev()
-    _run("vae_image_to_nchw", lib().ddpo_vae_image_to_nchw(_p(img_nhwc), _p(out_nchw), b, h, w, _stream()), 0.0, _e)
+    _launch("vae_image_to_nchw", _p(img_nhwc), _p(out_nchw), b, h, w)
 
 
 def vae_encoder_head(x_nhwc, w, bias, wq, bq, moments, batch, h, wd, cin):
     _chk(moments, torch.float32, "moments")
-    _e = _ev()
-    _run("vae_encoder_head", lib().ddpo_vae_encoder_head(_p(x_nhwc), _p(w), _p(bias), _p(wq), _p(bq), _p(moments), batch, h,
-                                                         wd, cin, _stream()), 0.0, _e)
+    _launch("vae_encoder_head", _p(x_nhwc), _p(w), _p(bias), _p(wq), _p(bq), _p(moments), batch, h, wd, cin)
 
 
 def vae_conv_out(x_nhwc, w, bias, batch, h, wd, cin, raw_nchw=None, img_nhwc=None):
-    _e = _ev()
-    _run("vae_conv_out", lib().ddpo_vae_conv_out(_p(x_nhwc), _p(w), _p(bias), _p(raw_nchw), _p(img_nhwc), batch, h, wd,
-                                                 cin, _stream()), 0.0, _e)
+    _launch("vae_conv_out", _p(x_nhwc), _p(w), _p(bias), _p(raw_nchw), _p(img_nhwc), batch, h, wd, cin)
 
 
 # ------------------------------------------------------------ text encoder -------
@@ -700,24 +640,19 @@ def embed_tokens(ids, token_embedding, position_embedding, out, seq_len):
     _chk(ids, torch.int32, "ids")
     _chk(out, torch.float32, "out")
     rows, dim = out.shape
-    _e = _ev()
-    _run("embed_tokens", lib().ddpo_embed_tokens(_p(ids), _p(token_embedding), _p(position_embedding), _p(out), rows,
-                                                 int(seq_len), dim, token_embedding.shape[0], _stream()), 0.0, _e)
+    _launch("embed_tokens", _p(ids), _p(token_embedding), _p(position_embedding), _p(out), rows, int(seq_len), dim,
+            token_embedding.shape[0])
 
 
 def act_bf16(x, y_bf16, act):
     """act: "gelu" (erf form) or "quick_gelu"."""
     _chk(x, torch.float32, "x")
     _chk(y_bf16, torch.bfloat16, "y")
-    _e = _ev()
-    _run("act_bf16", lib().ddpo_act_bf16(_p(x), _p(y_bf16), x.numel(), {"gelu": 0, "quick_gelu": 1}[act], _stream()),
-         float(x.numel()) * 6, _e)
+    _launch("act_bf16", _p(x), _p(y_bf16), x.numel(), {"gelu": 0, "quick_gelu": 1}[act], work=float(x.numel()) * 6)
 
 
 def layernorm_f32(x, scale, bias, y, m, c, eps=1e-5):
-    _e = _ev()
-    _run("layernorm_f32", lib().ddpo_layernorm_f32(_p(x), _p(scale), _p(bias), _p(y), int(m), int(c), float(eps),
-                                                   _stream()), float(m) * c * 8, _e)
+    _launch("layernorm_f32", _p(x), _p(scale), _p(bias), _p(y), int(m), int(c), float(eps), work=float(m) * c * 8)
 
 
 # ------------------------------------------------------------ image tower --------
@@ -725,22 +660,18 @@ def patchify_bf16(img_nhwc, out_bf16, patch):
     _chk(img_nhwc, torch.float32, "img")
     _chk(out_bf16, torch.bfloat16, "out")
     b, s, _, _ = img_nhwc.shape
-    _e = _ev()
-    _run("patchify_bf16", lib().ddpo_patchify_bf16(_p(img_nhwc), _p(out_bf16), b, s, int(patch), out_bf16.shape[1],
-                                                   _stream()), 0.0, _e)
+    _launch("patchify_bf16", _p(img_nhwc), _p(out_bf16), b, s, int(patch), out_bf16.shape[1])
 
 
 def vit_tokens(patches, class_embedding, position_embedding, out, batch, n_patches, dim):
-    _e = _ev()
-    _run("vit_tokens", lib().ddpo_vit_tokens(_p(patches), _p(class_embedding), _p(position_embedding), _p(out), int(batch),
-                                             int(n_patches), int(dim), _stream()), 0.0, _e)
+    _launch("vit_tokens", _p(patches), _p(class_embedding), _p(position_embedding), _p(out), int(batch), int(n_patches),
+            int(dim))
 
 
 def l2norm_rows(x, y):
     _chk(x, torch.float32, "x")
     m, c = x.shape
-    _e = _ev()
-    _run("l2norm_rows", lib().ddpo_l2norm_rows(_p(x), _p(y), m, c, _stream()), 0.0, _e)
+    _launch("l2norm_rows", _p(x), _p(y), m, c)
 
 
 # ------------------------------------------------------------ LoRA adapters -------
@@ -751,14 +682,8 @@ def lora_merge(w, down, up, k, n, rank, fwd=None, ldk=0, row_offset=0, dgrad=Non
                scale=1.0):
     """bf16(w + scale down @ up) for w fp32 [k, n], down [k, rank], up [rank, n], into the forward operand layout of
     ``prep_weight`` (``fwd``) and / or the dgrad layout of ``prep_weight_dgrad`` (``dgrad``); ``merged``: the fp32 sum"""
-    _e = _ev()
-    _run("lora_merge", lib().ddpo_lora_merge(_p(w), int(k), int(n), _p(down), _p(up), int(rank), float(scale), _p(fwd),
-                                             int(ldk), int(row_offset), _p(dgrad), int(ld_dst), int(col_offset),
-                                             _p(merged), _stream()), 0.0, _e)
-
-
-_LORA_WS = {}
-_KERNELS_PER_CALL["lora_grad"] = 2
+    _launch("lora_merge", _p(w), int(k), int(n), _p(down), _p(up), int(rank), float(scale), _p(fwd), int(ldk),
+            int(row_offset), _p(dgrad), int(ld_dst), int(col_offset), _p(merged))
 
 
 def lora_grad(x, dys, downs, ups, d_downs, d_ups, m, k, n, rank, ldx=0, lddy=0, scale=1.0):
@@ -769,18 +694,12 @@ def lora_grad(x, dys, downs, ups, d_downs, d_ups, m, k, n, rank, ldx=0, lddy=0, 
     need = int(lib().ddpo_lora_grad_workspace_floats(int(rank), g, int(m), int(k), int(n)))
     if need < 0:
         raise ValueError(f"lora_grad: no tiling for k={k}, n={n}, {g} adapters at rank {rank}")
-    dev = x.device
-    ws = _LORA_WS.get(dev)
-    if ws is None or ws.numel() < need:
-        ws = torch.empty(max(need, 1 << 20), dtype=torch.float32, device=dev)
-        _LORA_WS[dev] = ws
+    ws = _workspace("lora_grad", x.device, need)
     arr = lambda ts: (C.c_void_p * g)(*[t.data_ptr() for t in ts])   # noqa: E731
     for t in list(dys) + [x]:
         assert t.is_cuda and t.dtype == torch.bfloat16
     for t in list(downs) + list(ups) + list(d_downs) + list(d_ups):
         assert t.is_cuda and t.dtype == torch.float32
-    _e = _ev()
-    _run("lora_grad", lib().ddpo_lora_grad(_p(x), int(ldx or k), arr(dys), int(lddy or n), arr(downs), arr(ups),
-                                           arr(d_downs), arr(d_ups), g, int(m), int(k), int(n), int(rank), float(scale),
-                                           _p(ws), ws.numel(), _stream()),
-         float(m) * (k + g * n) * 2, _e, f"M{m} K{k} N{n} G{g} r{rank}" if _e is not None else "")
+    _launch("lora_grad", _p(x), int(ldx or k), arr(dys), int(lddy or n), arr(downs), arr(ups), arr(d_downs), arr(d_ups),
+            g, int(m), int(k), int(n), int(rank), float(scale), _p(ws), ws.numel(), work=float(m) * (k + g * n) * 2,
+            tag=f"M{m} K{k} N{n} G{g} r{rank}" if PROFILE is not None else "")

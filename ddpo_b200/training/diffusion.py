@@ -24,6 +24,7 @@ import numpy as np
 import torch
 
 from .. import ops
+from ..ops import graph_step   # host-side control: stays the real one where ``ops`` is swapped for an emulator
 from . import distributed
 from .policy_gradient import AccumulatingTrainState, AdamWConfig  # noqa: F401  (same optimizer chain)
 from ..unet import UNet
@@ -55,8 +56,7 @@ class _StepGraph:
         self.loss = torch.zeros(1, device=dev)
         self.per_sample = torch.zeros(b, device=dev)
         self.ws = ops.rwr_workspace(b, dev)
-        self.graph = None
-        self.sig = None
+        self.graph = None   # what ops.graph_step returned
 
 
 _GRAPHS: Dict[Any, _StepGraph] = {}
@@ -137,20 +137,11 @@ def train_step(state: AccumulatingTrainState, text_encoder_params, batch, train_
         G.weights.copy_(wt.reshape(b).to(dev, torch.float32))
     ac = noise_scheduler_state.common.alphas_cumprod
     sig = (float(guidance_scale), id(ac))
-    if not USE_CUDA_GRAPH:
+
+    def body():
         _run_body(unet, G, b, bool(train_cfg), ac, guidance_scale)
-    else:
-        if G.graph is None or G.sig != sig:
-            saved = state.grad_acc.clone()   # warm-up outside capture; undo its gradient contribution
-            _run_body(unet, G, b, bool(train_cfg), ac, guidance_scale)
-            torch.cuda.synchronize()
-            state.grad_acc.copy_(saved)
-            del saved
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                _run_body(unet, G, b, bool(train_cfg), ac, guidance_scale)
-            G.graph, G.sig = g, sig
-        G.graph.replay()
+
+    G.graph = graph_step(G.graph, sig, body, USE_CUDA_GRAPH, protect=state.grad_acc)
     loss = G.loss.clone()
     distributed.pmean_(loss)                                   # :95
     if isinstance(state, TrainState):

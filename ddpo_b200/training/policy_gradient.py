@@ -25,6 +25,7 @@ from typing import Any, Dict, Union
 import torch
 
 from .. import ops
+from ..ops import graph_step   # host-side control: stays the real one where ``ops`` is swapped for an emulator
 from . import distributed
 from ..unet import UNet
 
@@ -141,8 +142,7 @@ class _StepGraph:
         self.dlogp = torch.empty(b, device=dev)
         self.info = torch.empty(3, device=dev)
         self.ws = ops.ddim_workspace(b, dev)
-        self.graph = None
-        self.sig = None
+        self.graph = None   # what ops.graph_step returned
 
 
 _GRAPHS: Dict[Any, _StepGraph] = {}
@@ -220,21 +220,11 @@ def train_step(state: AccumulatingTrainState, batch, noise_scheduler_state, nois
     assert b % mb == 0
     pred = noise_scheduler.config.prediction_type   # the reference branches on it inside scheduler.step (:303-321)
     sig = (float(guidance_scale), float(eta), float(clip_range), ratio, id(noise_scheduler_state.common.alphas_cumprod), mb, pred)
-    if not USE_CUDA_GRAPH:
+
+    def body():
         _run_body(unet, G, b, bool(train_cfg), noise_scheduler_state, ratio, guidance_scale, eta, clip_range, mb, pred)
-    else:
-        if G.graph is None or G.sig != sig:
-            # warm-up outside capture (arena, workspaces, kernel attributes); undo its gradient contribution
-            saved = state.grad_acc.clone()
-            _run_body(unet, G, b, bool(train_cfg), noise_scheduler_state, ratio, guidance_scale, eta, clip_range, mb, pred)
-            torch.cuda.synchronize()
-            state.grad_acc.copy_(saved)
-            del saved
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                _run_body(unet, G, b, bool(train_cfg), noise_scheduler_state, ratio, guidance_scale, eta, clip_range, mb, pred)
-            G.graph, G.sig = g, sig
-        G.graph.replay()
+
+    G.graph = graph_step(G.graph, sig, body, USE_CUDA_GRAPH, protect=state.grad_acc)
     info_t = G.info.clone()
     if pmean_info:
         distributed.pmean_(info_t)                                # lax.pmean(info) (:142)
