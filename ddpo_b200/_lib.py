@@ -26,7 +26,7 @@ class IGemmArgs(C.Structure):
                 ("m", i32), ("n", i32), ("wt", vp), ("bias", vp), ("rowvec", vp), ("rows_per_sample", i32),
                 ("rowvec_ld", i32), ("residual", vp), ("ld_res", i32), ("out_f32", vp), ("out_bf16", vp),
                 ("ld_out", i32), ("geglu", i32), ("accumulate_out", i32), ("bn_override", i32), ("aux_bf16", vp),
-                ("conv_pad", i32), ("gn_stats", vp)]
+                ("conv_pad", i32), ("gn_stats", vp), ("bm_override", i32)]
 
 
 class GroupNormArgs(C.Structure):
@@ -70,6 +70,7 @@ SIGNATURES = {
     "ddpo_ddim_logprob_bwd": (i32, [C.POINTER(DdimCommon), vp, vp, vp, vp, vp]),
     "ddpo_ppo_loss": (i32, [vp, vp, vp, i32, i32, f32, vp, vp, vp]),
     "ddpo_igemm": (i32, [C.POINTER(IGemmArgs), vp]),
+    "ddpo_igemm_plan": (i32, [i32, i32, i32, i32, i32, i32, vp]),
     "ddpo_groupnorm_workspace_floats": (i64, [i32, i32, i32]),
     "ddpo_groupnorm_fwd": (i32, [C.POINTER(GroupNormArgs), vp]),
     "ddpo_groupnorm_bwd": (i32, [C.POINTER(GroupNormArgs), vp, vp, vp, i32, i32, i32, vp, vp, vp]),

@@ -192,8 +192,9 @@ def ppo_loss(logp, old_logp, adv, clip_range, info_out, dlogp_out, micro_batch=N
 def igemm(*, a0, wt, n, a1=None, c0=None, c1=0, lda0=None, lda1=None, conv=None, m=None, taps=1, stride=1,
           bias=None, rowvec=None, rows_per_sample=0, rowvec_ld=0, residual=None, ld_res=0, out_f32=None,
           out_bf16=None, ld_out=0, geglu=False, accumulate=False, bn=0, aux_bf16=None, gn_stats=None,
-          no_low_pad=False):
-    """conv=(batch, h_out, w_out) for convolutions, else linear with m rows."""
+          no_low_pad=False, bm=0):
+    """conv=(batch, h_out, w_out) for convolutions, else linear with m rows.  ``bm`` / ``bn`` force the output tile's
+    height / width (tests; 0 = the library's plan, ``igemm_plan``)."""
     a = IGemmArgs()
     a.a0, a.a1 = _p(a0), _p(a1)
     a.c0 = int(c0 if c0 is not None else a0.shape[-1])
@@ -215,12 +216,20 @@ def igemm(*, a0, wt, n, a1=None, c0=None, c1=0, lda0=None, lda1=None, conv=None,
     a.aux_bf16 = _p(aux_bf16)
     a.gn_stats = _p(gn_stats)
     a.conv_pad = int(no_low_pad)
+    a.bm_override = int(bm)
     rows = a.batch * a.h * a.w if a.is_conv else a.m
     _launch("igemm", C.byref(a), work=2.0 * rows * a.n * a.taps * (a.c0 + a.c1),
             tag=f"M{rows} N{a.n} K{a.taps * (a.c0 + a.c1)} taps{a.taps} s{a.conv_stride}"
                 f"{' geglu' if geglu else ''}{' res' if residual is not None else ''}"
                 f"{' f32' if out_f32 is not None else ''}{' bf16' if out_bf16 is not None else ''}"
                 f"{' acc' if accumulate else ''}" if PROFILE is not None else "")
+
+
+def igemm_plan(m, n, k, geglu=False, bm=0, bn=0):
+    """(BM, BN, CTAs per SM, operand stages) of the tile ``igemm`` runs for an [m, k] x [k, n] product; host only."""
+    plan = (C.c_int * 4)()
+    check(lib().ddpo_igemm_plan(int(m), int(n), int(k), int(geglu), int(bm), int(bn), plan), "igemm_plan")
+    return tuple(plan)
 
 
 # ------------------------------------------------------------------ norms -------

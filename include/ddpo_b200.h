@@ -117,15 +117,19 @@ typedef struct {
   int ld_out;
   int geglu;                /* out_bf16[M, n/2] = lin * gelu_tanh(gate); weight rows tile-interleaved */
   int accumulate_out;       /* out_f32 += */
-  int bn_override;          /* 0 = auto; else the tile width: 32, 64, 96, 128, 160, 192, 256 */
+  int bn_override;          /* 0 = planned; else the tile width (tests): 32, 64, 96, 128, 160, 192, 256 */
   void* aux_bf16;           /* GEGLU only, optional: bf16 [M, n] pre-activation (tile-interleaved, bias included) */
   int conv_pad;             /* 0 = the 3x3 default (symmetric pad 1); 1 = NO low-side padding: out[y,x] = sum in[s y + dy, s x + dx],
                                reads past the high edge are zero -- the VAE encoder's down-sample (pad ((0,1),(0,1)) + VALID) */
   float* gn_stats;          /* optional, with out_f32: fp32 [ceil(M/32), n, 2] = per 32-row slab and output column the (sum, sum
                                of squares) of the values written to out_f32.  The GroupNorm that consumes out_f32 takes its
                                statistics from these (ddpo_groupnorm_args.stats0/1) instead of reading the tensor twice. */
+  int bm_override;          /* 0 = planned; else the tile height (tests): 64 or 128 */
 } ddpo_igemm_args;
 int ddpo_igemm(const ddpo_igemm_args* a, void* stream);
+/* The output tile ddpo_igemm runs for an [m, k] x [k, n] product (k = taps * (c0 + c1)): plan = {BM, BN, CTAs per SM,
+ * operand stages}.  A function of the shape alone; the overrides are those of ddpo_igemm_args.  No GPU needed. */
+int ddpo_igemm_plan(int m, int n, int k, int geglu, int bm_override, int bn_override, int* plan);
 
 /* ------------------------------------------------------------ normalisation --------
  * flax.linen.GroupNorm(32, eps 1e-5)(+nn.swish) / LayerNorm(eps 1e-5) of the 3P Flax U-Net
