@@ -46,7 +46,7 @@ class WgradArgs(C.Structure):
     _fields_ = [("dy", vp), ("ldy", i32), ("n", i32), ("x0", vp), ("x1", vp), ("c0", i32), ("c1", i32),
                 ("ldx0", i32), ("ldx1", i32), ("is_conv", i32), ("batch", i32), ("h", i32), ("w", i32),
                 ("conv_stride", i32), ("taps", i32), ("m", i32), ("dw", vp), ("workspace", vp),
-                ("workspace_floats", i64)]
+                ("workspace_floats", i64), ("bn_override", i32), ("splits_override", i32)]
 
 
 class AttentionBwdArgs(C.Structure):
@@ -94,6 +94,7 @@ SIGNATURES = {
     "ddpo_attention_fwd": (i32, [C.POINTER(AttentionArgs), vp]),
     "ddpo_wgrad_workspace_floats": (i64, [C.POINTER(WgradArgs)]),
     "ddpo_wgrad": (i32, [C.POINTER(WgradArgs), vp]),
+    "ddpo_wgrad_plan": (i32, [i32, i32, i32, i32, i32, i32, i32, vp]),
     "ddpo_attention_bwd": (i32, [C.POINTER(AttentionBwdArgs), vp]),
     "ddpo_colsum_workspace_floats": (i64, [i32, i32, i32]),
     "ddpo_colsum_cast": (i32, [vp, i32, vp, vp, i32, i32, vp, i32, i32, vp]),

@@ -170,6 +170,21 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
   }
 }
+// mbar_wait that returns false after the same timeout instead of trapping, for code after a setmaxnreg.inc: a trap
+// inside such a region makes ptxas allocate it as if the increase had not happened (and spill).  The caller traps once
+// it is out of the region's hot loop.
+__device__ __forceinline__ bool mbar_wait_timed(uint64_t* bar, uint32_t parity) {
+  long long t0 = 0;
+  uint32_t spins = 0;
+  while (!mbar_try_wait(bar, parity)) {
+    if ((++spins & 255u) == 0) {
+      const long long now = clock64();
+      if (t0 == 0) t0 = now;
+      else if (now - t0 > DDPO_MBAR_TIMEOUT_CYCLES) return false;
+    }
+  }
+  return true;
+}
 
 // -------------------------------------------------------------------- TMA ----
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {

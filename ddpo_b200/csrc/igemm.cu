@@ -25,6 +25,7 @@
 //    whatever (BM, BN) a launch gets (the PPO ratio of an unchanged policy must be exactly 1; reference
 //    config/base.py:88 clip 1e-4).
 #include "common.cuh"
+#include "gemm_model.cuh"
 #include "wgmma.cuh"
 
 namespace ddpo {
@@ -300,25 +301,13 @@ static int geglu_width(int N) {
   return 0;
 }
 
-// Cost model of one launch, in SM clock cycles of an H100 SXM.  Rates are per SM; the L2 rate (7.7 TB/s over the chip)
-// is the one that makes the model's choices agree with CUDA-event timings of every tile on the U-Net's launches
-// (tests/bench_igemm_plan.py --all), the others are data-sheet figures.
-constexpr int NUM_SMS = 132;
-constexpr double TENSOR_FLOP_PER_CLK = 4096.0;  // dense bf16 wgmma (989 TFLOP/s = 132 SMs x 1.83 GHz x 4096)
-constexpr double SMEM_BYTES_PER_CLK = 128.0;    // shared-memory bandwidth that feeds the wgmma operands
-constexpr double L2_BYTES_PER_CLK = 32.0;       // TMA operand loads out of L2
-constexpr double HBM_BYTES_PER_CLK = 14.0;      // 3.35 TB/s shared by 132 SMs at 1.83 GHz
+// Cost model of one launch (gemm_model.cuh), in SM clock cycles.
 constexpr double EPI_BYTES_PER_ELEM = 8.0;      // epilogue traffic per output element: an fp32 store plus one fp32 read
                                                 // (residual, accumulate) or bf16 store, typical of the U-Net's launches
-// Makespan = waves x the time of one wave.  A k16 step of a tile is paced by the slowest of: the tensor cores
-// (2*64*BN*16 FLOP per warpgroup), shared memory (each warpgroup reads 2 KB of A plus BN x 32 B of B: narrow tiles,
-// BN <= 64, are bound by it) and L2 ((BM + BN) x 32 B of operands per tile: low tiles re-read B, narrow ones A).  The
-// c CTAs of a wave share the SM: with c >= 2 one CTA's epilogue overlaps the others' main loops, with c = 1 it does not.
+// Makespan = waves x the time of one wave, a wave being K / 16 steps of k16_step_clk plus the epilogue.  The c CTAs
+// of a wave share the SM: with c >= 2 one CTA's epilogue overlaps the others' main loops, with c = 1 it does not.
 static double tile_makespan(const TileShape& t, int M, int N, int K) {
-  const double wgs = t.bm / 64;
-  const double step = fmax(fmax(wgs * 2.0 * 64 * t.bn * 16 / TENSOR_FLOP_PER_CLK, wgs * (2048.0 + 32.0 * t.bn) / SMEM_BYTES_PER_CLK),
-                           (t.bm + t.bn) * 32.0 / L2_BYTES_PER_CLK);
-  const double main_loop = (K / 16) * step;
+  const double main_loop = (K / 16) * k16_step_clk(t.bm, t.bn);
   const double epilogue = double(t.bm) * t.bn * EPI_BYTES_PER_ELEM / HBM_BYTES_PER_CLK;
   const double wave = t.ctas_per_sm > 1 ? t.ctas_per_sm * fmax(main_loop, epilogue) : main_loop + epilogue;
   const long long tiles = (long long)((M + t.bm - 1) / t.bm) * (N / t.bn);

@@ -352,8 +352,10 @@ def attention_fwd(q, k, v, out, batch, heads, nq, nk, ldq, ldk, ldv, ldo, lse=No
 
 
 # ------------------------------------------------------------------ wgrad -------
-def wgrad(*, dy, n, x0, dw, x1=None, c0=None, c1=0, ldy=0, ldx0=0, ldx1=0, conv=None, m=None, taps=1, stride=1):
-    """dw[(tap, cin), n] += X^T dY (fp32, Flax layout).  conv=(batch, h_out, w_out) or linear with m rows."""
+def wgrad(*, dy, n, x0, dw, x1=None, c0=None, c1=0, ldy=0, ldx0=0, ldx1=0, conv=None, m=None, taps=1, stride=1,
+          bn=0, splits=0):
+    """dw[(tap, cin), n] += X^T dY (fp32, Flax layout).  conv=(batch, h_out, w_out) or linear with m rows.  ``bn`` /
+    ``splits`` force the column-tile width / pixel split count (tests; 0 = the library's plan, ``wgrad_plan``)."""
     a = WgradArgs()
     a.dy, a.ldy, a.n = _p(dy), int(ldy), int(n)
     a.x0, a.x1 = _p(x0), _p(x1)
@@ -365,6 +367,7 @@ def wgrad(*, dy, n, x0, dw, x1=None, c0=None, c1=0, ldy=0, ldx0=0, ldx1=0, conv=
         a.is_conv, a.batch, a.h, a.w, a.m = 0, 0, 0, 0, int(m)
     a.conv_stride, a.taps = int(stride), int(taps)
     a.dw = _p(dw)
+    a.bn_override, a.splits_override = int(bn), int(splits)
     need = int(lib().ddpo_wgrad_workspace_floats(C.byref(a)))
     ws = _workspace("wgrad", dw.device, need) if need > 0 else None
     a.workspace = _p(ws)
@@ -372,6 +375,13 @@ def wgrad(*, dy, n, x0, dw, x1=None, c0=None, c1=0, ldy=0, ldx0=0, ldx1=0, conv=
     rows = a.batch * a.h * a.w if a.is_conv else a.m
     _launch("wgrad", C.byref(a), work=2.0 * rows * a.n * a.taps * (a.c0 + a.c1),
             tag=f"M{rows} N{a.n} K{a.taps * (a.c0 + a.c1)} taps{a.taps} s{a.conv_stride}" if PROFILE is not None else "")
+
+
+def wgrad_plan(m, c0, n, c1=0, taps=1, bn=0, splits=0):
+    """(BN, pixel splits) of the launch ``wgrad`` runs over m pixels (b*h*w of dY for convolutions); host only."""
+    plan = (C.c_int * 2)()
+    check(lib().ddpo_wgrad_plan(int(m), int(c0), int(c1), int(n), int(taps), int(bn), int(splits), plan), "wgrad_plan")
+    return tuple(plan)
 
 
 # ------------------------------------------------------- backward wrappers -------

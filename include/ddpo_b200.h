@@ -230,9 +230,14 @@ typedef struct {
   float* dw;       /* fp32 [taps*(c0+c1), n], accumulated */
   float* workspace;
   int64_t workspace_floats;
+  int bn_override;      /* 0 = planned; else the column-tile width (tests): 64, 128, 192, 256 or 320, dividing n */
+  int splits_override;  /* 0 = planned; else the number of pixel ranges summed separately (tests), 1 .. ceil(m / 64) */
 } ddpo_wgrad_args;
 int64_t ddpo_wgrad_workspace_floats(const ddpo_wgrad_args* a);
 int ddpo_wgrad(const ddpo_wgrad_args* a, void* stream);
+/* The launch ddpo_wgrad runs for m pixels (batch * h * w of dY for convolutions): plan = {column-tile width BN, pixel
+ * splits}.  A function of the shape alone; the overrides are those of ddpo_wgrad_args.  No GPU needed. */
+int ddpo_wgrad_plan(int m, int c0, int c1, int n, int taps, int bn_override, int splits_override, int* plan);
 
 /* attention backward (dQ, dK, dV; deterministic two-kernel scheme), see csrc/attention_bwd.cu.  Head dims, column
  * layout and alignment rules as for ddpo_attention_fwd (they apply to out, dout, dq, dk and dv too); the scale is
